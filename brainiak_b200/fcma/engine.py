@@ -19,20 +19,31 @@ from .. import _lib
 
 _PREC_DEFAULT = "fp32"
 
-# "fp32" (the default of the public classes) means fp32-faithful correlations (|dr| <= 1e-6) by the
-# fastest 3-product split: fp16 hi/lo planes (pre-scaled by 2^6, bf16 tensor speed) when the data is
-# in the normalised range the reference's contract guarantees (|x| <= 1, voxelselector.py:72-76),
-# tf32 hi/lo planes (any finite fp32 range) otherwise.
+# "fp32" (the default of the public classes) means fp32-faithful correlations (|dr| <= 1e-6 * |x_i| |x_j|) by
+# the fastest 3-product split: fp16 hi/lo planes (pre-scaled by 2^6, bf16 tensor speed) when the data is in the
+# normalised range the reference's contract guarantees (unit-norm voxels, voxelselector.py:72-76), tf32 hi/lo
+# planes (any finite fp32 range) otherwise.  The fp16 split is faithful only while the low plane stays a normal
+# fp16 number: an element below 2^-9 leaves it with an absolute quantum of 2^-31, i.e. an error of about
+# 2^-30 * sqrt(T) / min(|x_i|, |x_j|) in r.  So the data must have |x| <= 8 (no overflow of x * 2^6 and its products)
+# and every non-zero per-(epoch, voxel) L2 norm >= 1/8 (1.7e-7 at T = 500); all-zero voxels are exact either way.
 _FP16_SAFE_AMAX = 8.0
+_FP16_SAFE_MIN_NORM = 0.125
+_FP16_SCALE = 64.0                  # FCMA_FP16_SCALE of the packer
+_FP16_MAX = 65504.0
 
 
 def resolve_precision(precision, epochs=None, normalize=False):
+    """``"fp32"`` -> ``"fp16x3"`` where the fp16 split is fp32-faithful for ``epochs`` ([E, T, V]), else ``"tf32x3"``;
+    any other precision is returned unchanged.  ``normalize=True``: the packer's output is unit-norm or zero."""
     if precision != "fp32":
         return precision
     if normalize or epochs is None:
         return "fp16x3"
-    amax = float(epochs.abs().max())
-    return "fp16x3" if amax <= _FP16_SAFE_AMAX else "tf32x3"
+    vmax = torch.linalg.vector_norm(epochs, float("inf"), dim=1)      # [E, V]
+    norm = torch.linalg.vector_norm(epochs, 2, dim=1)
+    # a non-zero voxel whose squares underflow has norm 0 < 1/8 and is caught as well
+    unsafe = (vmax.max() > _FP16_SAFE_AMAX) | ((vmax > 0) & (norm < _FP16_SAFE_MIN_NORM)).any()
+    return "tf32x3" if bool(unsafe) else "fp16x3"
 
 
 def _stream_ptr():
@@ -139,6 +150,11 @@ def pack_epochs(epochs, T_e=None, precision=_PREC_DEFAULT, normalize=False, v_be
     if epochs.dtype != torch.float32 or not epochs.is_cuda or not epochs.is_contiguous():
         raise ValueError("epochs must be a contiguous float32 CUDA tensor [E, T, V]")
     E, T, V = epochs.shape
+    if precision == "fp16x3" and not normalize:
+        amax = float(torch.linalg.vector_norm(epochs, float("inf")))
+        if amax * _FP16_SCALE > _FP16_MAX:
+            raise ValueError("fp16x3 stores x * %g in fp16, which overflows for max |x| = %g (limit %g): use "
+                             "'tf32x3' or 'fp32'" % (_FP16_SCALE, amax, _FP16_MAX / _FP16_SCALE))
     precision = resolve_precision(precision, epochs, normalize)
     code = _prec_code(precision)
     if code == _lib.PREC["f32simt"]:

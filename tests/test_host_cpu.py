@@ -82,6 +82,42 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
         _lib.load()
 
 
+def test_resolve_precision_keeps_the_fp16_split_faithful():
+    """'fp32' takes the fp16 hi/lo split only for |x| <= 8 and per-(epoch, voxel) norms >= 1/8 (or 0): below that the
+    low plane goes subnormal and the split stops being fp32-faithful; tf32x3 otherwise.  CPU tensors, no device."""
+    import torch
+    rng = np.random.RandomState(3)
+    g = rng.randn(4, 200, 64)
+    unit = torch.from_numpy((g / np.linalg.norm(g, axis=1, keepdims=True)).astype(np.float32))
+    res = engine.resolve_precision
+    for s, want in ((8, "fp16x3"), (1, "fp16x3"), (0.25, "fp16x3"), (2.0 ** -4, "tf32x3"), (2.0 ** -8, "tf32x3"),
+                    (2.0 ** -12, "tf32x3"), (2.0 ** -16, "tf32x3"), (2.0 ** -20, "tf32x3")):
+        assert res("fp32", unit * s) == want, s
+    big = unit.clone()
+    big[1, 7, 3] = 8.5                                   # one element above the amax bound
+    assert res("fp32", big) == "tf32x3"
+    mixed = unit.clone()
+    mixed[:, :, 10:18] *= 2.0 ** -14                     # normalised data with 8 voxels at a small scale
+    assert res("fp32", mixed) == "tf32x3"
+    one = unit.clone()
+    one[2, :, 5] *= 2.0 ** -4                            # a single (epoch, voxel)
+    assert res("fp32", one) == "tf32x3"
+    tiny = unit.clone()
+    tiny[0, :, 0] = 1e-30                                # squares underflow to a zero norm: still non-zero data
+    assert res("fp32", tiny) == "tf32x3"
+    zero = unit.clone()
+    zero[:, :, :3] = 0                                   # all-zero voxels and (epoch, voxel) columns are exact
+    zero[1, :, 10] = 0
+    assert res("fp32", zero) == "fp16x3"
+    assert res("fp32", torch.zeros(2, 5, 7)) == "fp16x3"
+    # normalize=True: the packer's z-score makes every column unit-norm or zero, whatever the input scale
+    assert res("fp32", unit * 2.0 ** -20, normalize=True) == "fp16x3"
+    assert res("fp32", unit * 1e4, normalize=True) == "fp16x3"
+    # explicit precisions are never changed
+    for p in ("fp16x3", "tf32x3", "bf16x3", "tf32", "bf16"):
+        assert res(p, unit * 2.0 ** -20) == p
+
+
 def test_voxelselector_constructor_contract():
     raw, labels = synthetic.make_epochs(8, 6, 4)
     # voxelselector.py:130-134
