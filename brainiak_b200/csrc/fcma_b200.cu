@@ -408,6 +408,17 @@ __device__ __forceinline__ float fisher_fast(float r)
     return 0.34657359027997264f * (lg2_ftz(num) - lg2_ftz(den));
 }
 
+// mean^2 - E[x^2] of a subject's EPS values from nm = -mean and ns2 = -E[x^2], as one FMA.  EPS == 1: exactly 0, as in
+// fcma_extension.cc (x*x/1 - x*x); the FMA would return the rounding error of x^2, and its rsqrt z-scores of up to ~1
+template <int EPS>
+__device__ __forceinline__ float2 neg_variance(float2 nm, float2 ns2)
+{
+    if constexpr (EPS == 1)
+        return splat2(0.f);
+    else
+        return ffma2(nm, nm, ns2);
+}
+
 // GEMM-epilogue Fisher-z, series form: atanh(r) = r + r^3/3 + ... + r^13/13 for |r| <= 0.35 (truncation
 // < 3e-8 relative; 9 FMA-pipe ops, no MUFU).  The epilogue takes it for a whole warp block when no
 // element exceeds the bound (warp vote; r ~ N(0, 1/sqrt(T)) makes that the common case) and the
@@ -1318,7 +1329,7 @@ __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
                 auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
                     const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
                     mi = ffma2(nm, inv, splat2(0.f));
@@ -1539,7 +1550,7 @@ __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
 // cp.async into a swizzled smem buffer (double-buffered), warp w takes the 16-byte pieces of columns 4w .. 4w+3.
 // Lane (g, t) holds epochs 4g .. 4g+3 x rows {2t, 2t+1, 2t+8, 2t+9} x 4 columns; the rows are the k extent of
 // mma.m16n8k16 (fp16), one accumulator set per column (4 x 32 registers).  The within-subject z-score is the same
-// arithmetic as in k_norm_syrk (statistics over the epochs of a subject, packed fp32x2).  Every 128 row steps the
+// arithmetic as in k_norm_syrk (statistics over the epochs of a subject, packed fp32x2).  Every COLS_SEG_STEPS (64) row steps the
 // accumulators are folded into K through shared memory (bounds the truncating MMA accumulation chain, cf.
 // k_norm_syrk) with the symmetric mirror of cython_blas.pyx:200-207.
 // smem piece (line L = e*16 + row, 16-byte piece w) lives at (L*8 + (w ^ swz(L)))*16, swz(L) = ((L>>1)&3) | ((L>>6)&1)<<2:
@@ -1660,7 +1671,7 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                 auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
                     const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
                     mi = ffma2(nm, inv, splat2(0.f));
@@ -1923,7 +1934,7 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                 auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
                     const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
                     mi = ffma2(nm, inv, splat2(0.f));
@@ -2146,7 +2157,7 @@ __global__ void __launch_bounds__(256, 2)
                     for (int e = s0; e < s0 + EPS; e++) m = fadd2(m, v[e]), q2 = ffma2(v[e], v[e], q2);
                     const float2 nm = ffma2(m, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(q2, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     float2 inv;
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
@@ -2310,7 +2321,7 @@ __global__ void __launch_bounds__(256, 1)
                 auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
                     const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
                     mi = ffma2(nm, inv, splat2(0.f));
@@ -2584,7 +2595,7 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                 auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
                     const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
                     const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = ffma2(nm, nm, ns2);
+                    const float2 negvar = neg_variance<EPS>(nm, ns2);
                     inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
                     inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
                     mi = ffma2(nm, inv, splat2(0.f));

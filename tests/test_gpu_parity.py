@@ -328,7 +328,7 @@ def test_symmetric_column_pass_all_eps(dev, E, eps):
     work = engine.Workspace(E, V, 256, dev)            # the column-pass variant keeps only the block itself
     work.buf.view(torch.float32).fill_(float("nan"))
     engine.voxel_kernels_sym(op, 0, V, eps, flags=fl, work=work, out=K)      # 6 passes of <= 256 rows
-    # scale floor V: with eps = 1 every z-score is 0 in exact arithmetic (the kernels hold rounding residue ~1e-5 * V)
+    # scale floor V: with eps = 1 every z-score is 0 and so is K
     scale = max(float(plain.abs().max()), float(V))
     assert torch.isfinite(K).all()
     assert float((K - K.transpose(1, 2)).abs().max()) == 0.0
