@@ -9,8 +9,8 @@ SRC = os.path.join(HERE, "csrc", "fcma_b200.cu")
 DEPS = [SRC, os.path.join(HERE, "csrc", "ptx_sm90.cuh"),
         os.path.join(os.path.dirname(HERE), "include", "fcma_b200.h")]
 OUT = os.path.join(HERE, "libfcma_b200.so")
-# diagnostic build for tools/ only: same source with -DFCMA_DIAG, which compiles the A/B and debug knobs
-# (FCMA_SYM_COLS, FCMA_GEMM_STAGES, ...) in; the product library above never reads the environment
+# diagnostic build for tools/ only: same source with -DFCMA_DIAG, which compiles the A/B tuning knobs
+# (FCMA_GEMM_STAGES, FCMA_COLS_CPW, ...) in; the product library above never reads the environment
 OUT_DIAG = os.path.join(HERE, "libfcma_b200_diag.so")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -61,6 +61,28 @@ static int fail(int code, const char *fmt, ...)
 static inline long cdiv(long a, long b) { return (a + b - 1) / b; }
 static inline long round_up(long a, long b) { return cdiv(a, b) * b; }
 
+// Launches kernel<<<grid, block, smem, st>>>(args...) and counts it; a kernel that needs more than the default 48 KB of
+// dynamic shared memory gets its limit raised first.
+template <typename... Params, typename... Args>
+static int launch_kernel(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const char *name,
+                         Args... args)
+{
+    if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, block, smem, st>>>(args...);
+    LAUNCH_CHECK(name);
+    return FCMA_OK;
+}
+
+// Calls f(IntC<V>{}) for the V of the list that equals `value`, so that a kernel template is instantiated for exactly the
+// listed values.  Returns false when the list has no such V.
+template <int V>
+using IntC = std::integral_constant<int, V>;
+template <int... Vs, typename F>
+static bool with_int(int value, F &&f)
+{
+    return ((value == Vs && (f(IntC<Vs>{}), true)) || ...);
+}
+
 // Tuning / diagnostic knobs (A/B switches of tools/) exist only in the diagnostic build (-DFCMA_DIAG -> libfcma_b200_diag.so, `python -m brainiak_b200.build --diag`).  The
 // product library never reads the environment: a stray variable cannot change its numerics or layout.
 #ifdef FCMA_DIAG
@@ -170,7 +192,7 @@ struct PrecInfo {
 };
 // fp16 planes hold x * 2^6: |x| <= 1 for normalised epochs, so hi <= 64 and the low plane
 // (~2^-11 of hi) stays a NORMAL fp16 number down to |x| ~ 4e-3; the epilogue multiplies by 2^-12.
-#define FCMA_FP16_SCALE 64.0f
+constexpr float FCMA_FP16_SCALE = 64.0f;
 static bool prec_info(int precision, PrecInfo *p)
 {
     switch (precision) {
@@ -848,20 +870,12 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
         const char *gp = diag_env("FCMA_GEMM_PAIRS");
         if (gp && atoi(gp) >= 1 && atoi(gp) < pairs) pairs = atoi(gp);
     }
-#define FCMA_LAUNCH_GEMM(FF, HH)                                                                                      \
-    do {                                                                                                              \
-        CUDA_TRY(cudaFuncSetAttribute(k_corr_wgmma<FF, HH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k_corr_wgmma<FF, HH><<<(unsigned)(2 * pairs), GEMM_THREADS, smem, st>>>(tm_cols, tm_rows, q);             \
-    } while (0)
-    if (pi.fmt == 0) {
-        if (half_out) FCMA_LAUNCH_GEMM(0, true); else FCMA_LAUNCH_GEMM(0, false);
-    } else if (pi.fmt == 1) {
-        if (half_out) FCMA_LAUNCH_GEMM(1, true); else FCMA_LAUNCH_GEMM(1, false);
-    } else {
-        if (half_out) FCMA_LAUNCH_GEMM(2, true); else FCMA_LAUNCH_GEMM(2, false);
-    }
-#undef FCMA_LAUNCH_GEMM
-    LAUNCH_CHECK("k_corr_wgmma");
+    auto gemm = [&](auto kernel) {
+        rc = launch_kernel(kernel, (unsigned)(2 * pairs), GEMM_THREADS, smem, st, "k_corr_wgmma", tm_cols, tm_rows, q);
+    };
+    if (!with_int<0, 1, 2>(pi.fmt, [&](auto FMT) { half_out ? gemm(k_corr_wgmma<FMT, true>) : gemm(k_corr_wgmma<FMT, false>); }))
+        return fail(FCMA_EINVAL, "internal: no k_corr_wgmma instantiation for operand type %d", pi.fmt);
+    if (rc) return rc;
 
     if (rows_op == cols_op && V == V2 && fixup) {
         // self-correlation: replace the diagonal by the reference-exact values kept with the operand
@@ -2738,48 +2752,6 @@ __global__ void k_scale(float *x, long n, float s)
         x[i] = s == 0.f ? 0.f : x[i] * s;
 }
 
-template <int R, bool FISHER, int VEC>
-static bool dispatch_eps(int eps, dim3 grid, cudaStream_t st, const float *C, long nb, int E, long n2, long stride_i,
-                         long ld, long chunk_step, long self_col0, float beta, float *K, int sum, long rb_stride, double *K64)
-{
-    constexpr size_t smem = (VEC ? (size_t)8 * 2 * (VEC == 2 ? R : 2 * R) * 32 * sizeof(float4) : 0) +
-                            (R <= 4 ? (size_t)8 * (8 * R) * (8 * R) * sizeof(float) : 0);
-#define FCMA_CASE(EPSV)                                                                                          \
-    case EPSV:                                                                                                   \
-        if (smem > 48 * 1024)                                                                                    \
-            cudaFuncSetAttribute(k_norm_syrk<R, EPSV, FISHER, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                 (int)smem);                                                                     \
-        k_norm_syrk<R, EPSV, FISHER, VEC><<<grid, 256, smem, st>>>(C, nb, E, n2, stride_i, ld, chunk_step, self_col0, beta, K, sum, rb_stride, K64); \
-        return true;
-    switch (eps) {
-        FCMA_CASE(0)
-        FCMA_CASE(1)
-        FCMA_CASE(2)
-        FCMA_CASE(4)
-        FCMA_CASE(8)
-        FCMA_CASE(16)
-    case 32:
-        if constexpr (R >= 4) {      // R = 2 (E <= 16): a subject never spans 32 epochs
-            if (smem > 48 * 1024)
-                cudaFuncSetAttribute(k_norm_syrk<R, 32, FISHER, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            k_norm_syrk<R, 32, FISHER, VEC><<<grid, 256, smem, st>>>(C, nb, E, n2, stride_i, ld, chunk_step, self_col0, beta, K, sum, rb_stride, K64);
-            return true;
-        }
-        return false;
-    case 64:
-        if constexpr (R == 8) {
-            if (smem > 48 * 1024)
-                cudaFuncSetAttribute(k_norm_syrk<R, 64, FISHER, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem);
-            k_norm_syrk<R, 64, FISHER, VEC><<<grid, 256, smem, st>>>(C, nb, E, n2, stride_i, ld, chunk_step, self_col0, beta, K, sum, rb_stride, K64);
-            return true;
-        }
-        return false;
-    default: return false;
-    }
-#undef FCMA_CASE
-}
-
 // eps_mode: 0 = plain SYRK of normalised data; > 0 = fused normalisation with that eps
 static bool fused_supported(int E, int eps_mode)
 {
@@ -2814,33 +2786,34 @@ static int launch_norm_syrk(const float *C, long nb, int E, long n2, long stride
         return fail(FCMA_EINVAL, "internal: the fp16 block is tiled and already Fisher-transformed");
     // rows cost the same: a static stride over 16 blocks per SM balances well
     long g = nb < 16L * g_sm_count ? nb : 16L * g_sm_count;
-    dim3 grid((unsigned)g);
+    int rc = FCMA_OK;
+    // k_norm_syrk<R, EPS, FISHER, VEC> holds 8R padded epochs: it is built for EPS = 0 (plain SYRK) and every power of two
+    // up to 8R
+    auto run = [&](auto R, auto FISHER, auto VEC) {
+        constexpr size_t smem = (VEC ? (size_t)8 * 2 * (VEC == 2 ? R : 2 * R) * 32 * sizeof(float4) : 0) +
+                                (R <= 4 ? (size_t)8 * (8 * R) * (8 * R) * sizeof(float) : 0);
+        auto go = [&](auto EPS) {
+            rc = launch_kernel(k_norm_syrk<R, EPS, FISHER, VEC>, (unsigned)g, 256, smem, st, "k_norm_syrk", C, nb, E, n2,
+                               stride_i, ld, chunk_step, self_col0, beta, K, sum_over_rows, rb_stride, K64);
+        };
+        if constexpr (R == 2) return with_int<0, 1, 2, 4, 8, 16>(eps_mode, go);
+        else if constexpr (R == 4) return with_int<0, 1, 2, 4, 8, 16, 32>(eps_mode, go);
+        else return with_int<0, 1, 2, 4, 8, 16, 32, 64>(eps_mode, go);
+    };
+    auto per_layout = [&](auto R) {   // VEC: 0 scalar loads, 1 cp.async of an fp32 block, 2 of an fp16 block
+        if (half_in) return run(R, std::false_type{}, IntC<2>{});
+        if (fisher) return vec ? run(R, std::true_type{}, IntC<1>{}) : run(R, std::true_type{}, IntC<0>{});
+        return vec ? run(R, std::false_type{}, IntC<1>{}) : run(R, std::false_type{}, IntC<0>{});
+    };
     bool ok;
-#define FCMA_DISPATCH(RR, FI, VV) \
-    dispatch_eps<RR, FI, VV>(eps_mode, grid, st, C, nb, E, n2, stride_i, ld, chunk_step, self_col0, beta, K, sum_over_rows, rb_stride, K64)
-    if (E <= 16 && eps_mode <= 16 && !half_in && !fisher && vec) {
+    if (E <= 16 && eps_mode <= 16 && !half_in && !fisher && vec)
         // 16 padded epochs instead of 32 (lane = 2 epochs): half the statistics and MMA work per byte of the pipelines'
         // fp32 block (BASELINE configs[1]: E = 16)
-        ok = FCMA_DISPATCH(2, false, 1);
-    } else if (E <= 32) {
-        if (half_in)
-            ok = FCMA_DISPATCH(4, false, 2);
-        else if (fisher)
-            ok = vec ? FCMA_DISPATCH(4, true, 1) : FCMA_DISPATCH(4, true, 0);
-        else
-            ok = vec ? FCMA_DISPATCH(4, false, 1) : FCMA_DISPATCH(4, false, 0);
-    } else {
-        if (half_in)
-            ok = FCMA_DISPATCH(8, false, 2);
-        else if (fisher)
-            ok = vec ? FCMA_DISPATCH(8, true, 1) : FCMA_DISPATCH(8, true, 0);
-        else
-            ok = vec ? FCMA_DISPATCH(8, false, 1) : FCMA_DISPATCH(8, false, 0);
-    }
-#undef FCMA_DISPATCH
+        ok = run(IntC<2>{}, std::false_type{}, IntC<1>{});
+    else
+        ok = E <= 32 ? per_layout(IntC<4>{}) : per_layout(IntC<8>{});
     if (!ok) return fail(FCMA_EINVAL, "internal: no k_norm_syrk instantiation for E=%d eps=%d", E, eps_mode);
-    LAUNCH_CHECK("k_norm_syrk");
-    return FCMA_OK;
+    return rc;
 }
 
 // column-direction pass over a tiled fp32 block (k_norm_syrk_cols): K[j] += ... for block columns [c0, n2)
@@ -2852,29 +2825,18 @@ static int launch_norm_syrk_cols(const void *A, long n, int E, long n2, long T25
                                  cudaStream_t st, int half_in = 0, bool use_tma = false, bool v2 = false, bool pad32 = false)
 {
     if (!cols_supported(E, eps) || (c0 & 31) || c0 >= n2) return fail(FCMA_EINVAL, "internal: column pass unsupported E=%d eps=%d c0=%ld", E, eps, c0);
+    const float *A32 = reinterpret_cast<const float *>(A);
+    int rc = FCMA_OK;
     if (E > 32) {   // 32 < E <= 64, fp32 block: one column per warp, 8-column strips (k_norm_syrk_cols64)
         if (half_in) return fail(FCMA_EINVAL, "internal: no column pass over an fp16 block for E=%d", E);
         const long nstrips8 = cdiv(n2 - c0, 8);
         const unsigned grid64 = (unsigned)(nstrips8 < g_sm_count ? nstrips8 : g_sm_count);
         const size_t smem64 = (size_t)8 * 64 * 64 * sizeof(float) + 128;   // the fold area; the 3 bricks (102 KB) lie inside it
-#define FCMA_COLS64_CASE(EPSV)                                                                                      \
-    case EPSV:                                                                                                      \
-        CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols64<EPSV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem64)); \
-        k_norm_syrk_cols64<EPSV><<<grid64, 256, smem64, st>>>(reinterpret_cast<const float *>(A), n, E, n2, T256, c0, K); \
-        break;
-        switch (eps) {
-            FCMA_COLS64_CASE(1)
-            FCMA_COLS64_CASE(2)
-            FCMA_COLS64_CASE(4)
-            FCMA_COLS64_CASE(8)
-            FCMA_COLS64_CASE(16)
-            FCMA_COLS64_CASE(32)
-            FCMA_COLS64_CASE(64)
-        default: return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols64 instantiation for eps=%d", eps);
-        }
-#undef FCMA_COLS64_CASE
-        LAUNCH_CHECK("k_norm_syrk_cols64");
-        return FCMA_OK;
+        if (!with_int<1, 2, 4, 8, 16, 32, 64>(eps, [&](auto EPS) {
+                rc = launch_kernel(k_norm_syrk_cols64<EPS>, grid64, 256, smem64, st, "k_norm_syrk_cols64", A32, n, E, n2, T256, c0, K);
+            }))
+            return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols64 instantiation for eps=%d", eps);
+        return rc;
     }
     const long nstrips = cdiv(n2 - c0, 32);
     const unsigned grid = (unsigned)(nstrips < g_sm_count ? nstrips : g_sm_count);
@@ -2883,122 +2845,64 @@ static int launch_norm_syrk_cols(const void *A, long n, int E, long n2, long T25
     // bar.sync; opt-in, the cp.async kernel below stays the default.
     if (use_tma && (E & 3) == 0 && ((uintptr_t)K & 15) == 0 && ((uintptr_t)A & 15) == 0) {
         CUtensorMap tmA;
-        int rc = make_cols_map(&tmA, A, (size_t)cdiv(n, 256) * (size_t)T256, E, half_in);
+        rc = make_cols_map(&tmA, A, (size_t)cdiv(n, 256) * (size_t)T256, E, half_in);
         if (rc) return rc;
         const size_t smem_t = 196608 + 64 + 1024;
-#define FCMA_COLS_TMA_CASE(EPSV)                                                                                    \
-    case EPSV:                                                                                                      \
-        if (half_in) {                                                                                              \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols_tma<EPSV, true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t)); \
-            k_norm_syrk_cols_tma<EPSV, true, 4><<<grid, 256, smem_t, st>>>(tmA, (int)n, E, (int)n2, (int)T256, (int)c0, K); \
-        } else {                                                                                                    \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols_tma<EPSV, false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t)); \
-            k_norm_syrk_cols_tma<EPSV, false, 4><<<grid, 256, smem_t, st>>>(tmA, (int)n, E, (int)n2, (int)T256, (int)c0, K); \
-        }                                                                                                           \
-        break;
-        switch (eps) {
-            FCMA_COLS_TMA_CASE(1)
-            FCMA_COLS_TMA_CASE(2)
-            FCMA_COLS_TMA_CASE(4)
-            FCMA_COLS_TMA_CASE(8)
-            FCMA_COLS_TMA_CASE(16)
-            FCMA_COLS_TMA_CASE(32)
-        default: return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols_tma instantiation for eps=%d", eps);
-        }
-#undef FCMA_COLS_TMA_CASE
-        LAUNCH_CHECK("k_norm_syrk_cols_tma");
-        return FCMA_OK;
+        auto go = [&](auto kernel) {
+            rc = launch_kernel(kernel, grid, 256, smem_t, st, "k_norm_syrk_cols_tma", tmA, (int)n, E, (int)n2, (int)T256, (int)c0, K);
+        };
+        if (!with_int<1, 2, 4, 8, 16, 32>(eps, [&](auto EPS) {
+                half_in ? go(k_norm_syrk_cols_tma<EPS, true, 4>) : go(k_norm_syrk_cols_tma<EPS, false, 4>);
+            }))
+            return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols_tma instantiation for eps=%d", eps);
+        return rc;
     }
     // E <= 16 (fp32 block): 16-epoch bricks, two CTAs per SM (k_norm_syrk_cols16); the kernels below pad to 32 epochs
     if (!half_in && E <= 16 && eps <= 16 && !use_tma && !v2 && !pad32) {
         const size_t smem16 = (size_t)COLS_BRICKS * 32768 + 16384 + 128;
         const unsigned grid16 = (unsigned)(nstrips < 2L * g_sm_count ? nstrips : 2L * g_sm_count);
-#define FCMA_COLS16_CASE(EPSV)                                                                                      \
-    case EPSV:                                                                                                      \
-        CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols16<EPSV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16)); \
-        k_norm_syrk_cols16<EPSV><<<grid16, 256, smem16, st>>>(reinterpret_cast<const float *>(A), n, E, n2, T256, c0, K); \
-        break;
-        switch (eps) {
-            FCMA_COLS16_CASE(1)
-            FCMA_COLS16_CASE(2)
-            FCMA_COLS16_CASE(4)
-            FCMA_COLS16_CASE(8)
-            FCMA_COLS16_CASE(16)
-        default: return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols16 instantiation for eps=%d", eps);
-        }
-#undef FCMA_COLS16_CASE
-        LAUNCH_CHECK("k_norm_syrk_cols16");
-        return FCMA_OK;
+        if (!with_int<1, 2, 4, 8, 16>(eps, [&](auto EPS) {
+                rc = launch_kernel(k_norm_syrk_cols16<EPS>, grid16, 256, smem16, st, "k_norm_syrk_cols16", A32, n, E, n2, T256, c0, K);
+            }))
+            return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols16 instantiation for eps=%d", eps);
+        return rc;
     }
     // FCMA_FLAG_COLS_V2: thread-per-row normalisation, fp16 staging, ldmatrix fragments (k_norm_syrk_cols2, fp32 block).
     // ~2x fewer instructions than the fragment-layout kernel below; the column pass is bound by what it moves, not by
     // what it issues.  Opt-in, tested.
     if (!half_in && v2) {
         const size_t smem2 = (size_t)COLS_BRICKS * 65536 + 32768 + 1024;
-        // diagnostic build only: FCMA_COLS_V2_CPW=2 = 16 warps x 2 columns (A/B)
-        const char *c2_env = diag_env("FCMA_COLS_V2_CPW");
-        const bool v2_cpw2 = c2_env && c2_env[0] == '2';
+        auto go = [&](auto kernel, unsigned threads) {
+            rc = launch_kernel(kernel, grid, threads, smem2, st, "k_norm_syrk_cols2", A32, n, E, n2, T256, c0, K);
+        };
+        if (!with_int<1, 2, 4, 8, 16, 32>(eps, [&](auto EPS) {
 #ifdef FCMA_DIAG
-#define FCMA_COLS2_CPW2(EPSV)                                                                                       \
-    CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols2<EPSV, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2)); \
-    k_norm_syrk_cols2<EPSV, 2><<<grid, 512, smem2, st>>>(reinterpret_cast<const float *>(A), n, E, n2, T256, c0, K);
-#else
-#define FCMA_COLS2_CPW2(EPSV)
+                // FCMA_COLS_V2_CPW=2: 16 warps x 2 columns (A/B)
+                const char *cpw = diag_env("FCMA_COLS_V2_CPW");
+                if (cpw && cpw[0] == '2') return go(k_norm_syrk_cols2<EPS, 2>, 512);
 #endif
-#define FCMA_COLS2_CASE(EPSV)                                                                                       \
-    case EPSV:                                                                                                      \
-        if (v2_cpw2) {                                                                                              \
-            FCMA_COLS2_CPW2(EPSV)                                                                                   \
-        } else {                                                                                                    \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols2<EPSV, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2)); \
-            k_norm_syrk_cols2<EPSV, 4><<<grid, 256, smem2, st>>>(reinterpret_cast<const float *>(A), n, E, n2, T256, c0, K); \
-        }                                                                                                           \
-        break;
-        switch (eps) {
-            FCMA_COLS2_CASE(1)
-            FCMA_COLS2_CASE(2)
-            FCMA_COLS2_CASE(4)
-            FCMA_COLS2_CASE(8)
-            FCMA_COLS2_CASE(16)
-            FCMA_COLS2_CASE(32)
-        default: return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols2 instantiation for eps=%d", eps);
-        }
-#undef FCMA_COLS2_CASE
-#undef FCMA_COLS2_CPW2
-        LAUNCH_CHECK("k_norm_syrk_cols2");
-        return FCMA_OK;
+                go(k_norm_syrk_cols2<EPS, 4>, 256);
+            }))
+            return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols2 instantiation for eps=%d", eps);
+        return rc;
     }
     // bricks (3 x 64 KB fp32 / 3 x 32 KB fp16); the fold buffer [32 columns][32*32] fp32 = 128 KB overlays them
     const size_t smem = (half_in ? (size_t)131072 : (size_t)COLS_BRICKS * 65536) + 1024;
-    // 4 columns per warp (8 warps, 255 registers) by default; FCMA_COLS_CPW=2 selects 2 columns per warp (16 warps at 128
-    // registers, with spills and two-way conflicts on the 8-byte LDS; A/B)
-    const char *cpw_env = diag_env("FCMA_COLS_CPW");
-    const bool cpw4 = !(cpw_env && cpw_env[0] == '2');
-#define FCMA_COLS_CASE(EPSV)                                                                                        \
-    case EPSV:                                                                                                      \
-        if (half_in) {                                                                                              \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols<EPSV, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            k_norm_syrk_cols<EPSV, 4, true><<<grid, 256, smem, st>>>(A, n, E, n2, T256, c0, K);                    \
-        } else if (cpw4) {                                                                                          \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols<EPSV, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            k_norm_syrk_cols<EPSV, 4, false><<<grid, 256, smem, st>>>(A, n, E, n2, T256, c0, K);                   \
-        } else {                                                                                                    \
-            CUDA_TRY(cudaFuncSetAttribute(k_norm_syrk_cols<EPSV, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            k_norm_syrk_cols<EPSV, 2, false><<<grid, 512, smem, st>>>(A, n, E, n2, T256, c0, K);                   \
-        }                                                                                                           \
-        break;
-    switch (eps) {
-        FCMA_COLS_CASE(1)
-        FCMA_COLS_CASE(2)
-        FCMA_COLS_CASE(4)
-        FCMA_COLS_CASE(8)
-        FCMA_COLS_CASE(16)
-        FCMA_COLS_CASE(32)
-    default: return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols instantiation for eps=%d", eps);
-    }
-#undef FCMA_COLS_CASE
-    LAUNCH_CHECK("k_norm_syrk_cols");
-    return FCMA_OK;
+    auto go = [&](auto kernel, unsigned threads) {
+        rc = launch_kernel(kernel, grid, threads, smem, st, "k_norm_syrk_cols", A, n, E, n2, T256, c0, K);
+    };
+    if (!with_int<1, 2, 4, 8, 16, 32>(eps, [&](auto EPS) {
+            if (half_in) return go(k_norm_syrk_cols<EPS, 4, true>, 256);
+#ifdef FCMA_DIAG
+            // 4 columns per warp (8 warps, 255 registers) by default; FCMA_COLS_CPW=2 selects 2 columns per warp (16 warps
+            // at 128 registers, with spills and two-way conflicts on the 8-byte LDS; A/B)
+            const char *cpw = diag_env("FCMA_COLS_CPW");
+            if (cpw && cpw[0] == '2') return go(k_norm_syrk_cols<EPS, 2, false>, 512);
+#endif
+            go(k_norm_syrk_cols<EPS, 4, false>, 256);
+        }))
+        return fail(FCMA_EINVAL, "internal: no k_norm_syrk_cols instantiation for eps=%d", eps);
+    return rc;
 }
 
 // ============================================================================================
@@ -3127,11 +3031,9 @@ static int launch_syrk_simt(const float *z, long nb, int E, long n2, long stride
     }
     size_t smem = (size_t)64 * (E + 1) * sizeof(float);
     if (smem > 200 * 1024) return fail(FCMA_EINVAL, "E=%d too large for the SIMT kernel-matrix path", E);
-    if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(k_syrk_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     long g = nb < 148L * 8 ? nb : 148L * 8;
-    k_syrk_simt<<<(unsigned)g, 256, smem, st>>>(z, nb, E, n2, stride_i, ld, beta, K, sum_over_rows);
-    LAUNCH_CHECK("k_syrk_simt");
-    return FCMA_OK;
+    return launch_kernel(k_syrk_simt, (unsigned)g, 256, smem, st, "k_syrk_simt", z, nb, E, n2, stride_i, ld, beta, K,
+                         sum_over_rows);
 }
 
 extern "C" int fcma_kernel_matrices(const float *z_dev, long nb, int E, long n2, long stride_i, long ld, float beta,
@@ -3190,6 +3092,60 @@ extern "C" long fcma_timing_read(double *gemm_ms, double *syrk_ms)
     if (syrk_ms) *syrk_ms = g_t_syrk;
     return g_t_passes;
 }
+// Events of one pipeline pass while timing is on (each call records one on `st`; all do nothing while it is off).  end()
+// waits for the pass and adds GEMM = start..gemm_done, SYRK = gemm_done..end and, if rows_done() was called, SYRK2 =
+// rows_done..end to the totals.
+class PassTimer {
+    EventSet<4> evs;   // start, GEMM done, end, rows done
+    cudaStream_t st;
+    bool rows = false;
+    int record(int k)
+    {
+        if (evs.on) CUDA_TRY(cudaEventRecord(evs.ev[k], st));
+        return FCMA_OK;
+    }
+
+public:
+    explicit PassTimer(cudaStream_t s) : st(s) {}
+    int start()
+    {
+        if (!g_timing_on) return FCMA_OK;
+        CUDA_TRY(evs.create());
+        return record(0);
+    }
+    int gemm_done() { return record(1); }
+    int rows_done()
+    {
+        rows = true;
+        return record(3);
+    }
+    int end()
+    {
+        if (!evs.on) return FCMA_OK;
+        CUDA_TRY(cudaEventRecord(evs.ev[2], st));
+        CUDA_TRY(cudaEventSynchronize(evs.ev[2]));
+        float gemm = 0.f, syrk = 0.f, syrk2 = 0.f;
+        CUDA_TRY(cudaEventElapsedTime(&gemm, evs.ev[0], evs.ev[1]));
+        CUDA_TRY(cudaEventElapsedTime(&syrk, evs.ev[1], evs.ev[2]));
+        if (rows) CUDA_TRY(cudaEventElapsedTime(&syrk2, evs.ev[3], evs.ev[2]));
+        g_t_gemm += gemm, g_t_syrk += syrk, g_t_syrk2 += syrk2, g_t_passes++;
+        return FCMA_OK;
+    }
+};
+
+// Fisher-z block of the fused pipelines in fp16 rather than fp32: FCMA_FLAG_F16_INTERMEDIATE asks for it, and the
+// single-product reduced-precision operand modes (bf16 / tf32) take it by default.  The fp16 values' rounding errors are
+// independent across the V2 columns the kernel matrix sums over: measured max|dK|/max|K| = 1.5e-5 at V2 = 50 000 (the
+// reference's own fp32 ssyrk rounding noise is 1e-5), while both kernels move half the bytes (-8..12 % per step).  The
+// fp32-faithful modes keep an fp32 block unless the flag asks otherwise; correlation values returned by fcma_corr_block
+// are never rounded.  Diagnostic build: FCMA_F16_INTERMEDIATE=0|1 overrides (A/B).
+static bool half_block(int precision, int flags)
+{
+    bool half = (flags & FCMA_FLAG_F16_INTERMEDIATE) || precision == FCMA_PREC_BF16 || precision == FCMA_PREC_TF32;
+    const char *f16i = diag_env("FCMA_F16_INTERMEDIATE");
+    if (f16i && (f16i[0] == '0' || f16i[0] == '1')) half = f16i[0] == '1';
+    return half;
+}
 
 // shared body of the two fused pipelines
 static int run_pipeline(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2, long start,
@@ -3216,31 +3172,16 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
     // Tiled intermediate [n/256][T256][E][256][256]: every 256x256 pair tile of the GEMM is one contiguous 256 KB
     // run and the E tiles of one (row block, column block) are adjacent, so the fused normalise+SYRK kernel reads
     // row i as E runs of 1 KB, 256 KB apart, inside one 8 MB region.  Needs whole 256-row blocks of workspace.
-    // FCMA_NO_TILED=1 falls back to the strided [i][e][j] block.
-    const char *no_tiled = diag_env("FCMA_NO_TILED");
+    // FCMA_FLAG_STRIDED_BLOCK keeps the strided [i][e][j] block.
     const long t256 = cdiv(V2, 256);
-    const bool tiled = !(no_tiled && no_tiled[0] == '1') && !(flags & FCMA_FLAG_STRIDED_BLOCK) && fused &&
-                       V2 < (1L << 31) && rows_per_pass >= 256;
-    // fp16 intermediate (FCMA_FLAG_F16_INTERMEDIATE, and by default in the single-product reduced-precision operand
-    // modes bf16 / tf32): the tiled block holds Fisher-z values rounded to fp16.  Their rounding errors
-    // are independent across the V2 columns the kernel matrix sums over: measured max|dK|/max|K| = 1.5e-5 at
-    // V2 = 50 000 (the reference's own fp32 ssyrk rounding noise is 1e-5), while both kernels move half the
-    // bytes (-8..12 % per step).  The fp32-faithful modes keep an fp32 block unless the flag asks otherwise;
-    // correlation values returned by fcma_corr_block are never rounded.  FCMA_F16_INTERMEDIATE=0|1 overrides (A/B).
-    const char *f16i = diag_env("FCMA_F16_INTERMEDIATE");
-    const bool reduced = precision == FCMA_PREC_BF16 || precision == FCMA_PREC_TF32;
-    bool half16 = (flags & FCMA_FLAG_F16_INTERMEDIATE) || reduced;
-    if (f16i && (f16i[0] == '0' || f16i[0] == '1')) half16 = f16i[0] == '1';
-    half16 = half16 && tiled && normalise && fisher_in_gemm;
+    const bool tiled = !(flags & FCMA_FLAG_STRIDED_BLOCK) && fused && V2 < (1L << 31) && rows_per_pass >= 256;
+    // an fp16 block needs the tiled layout and holds Fisher-z values (applied in the GEMM epilogue)
+    const bool half16 = half_block(precision, flags) && tiled && normalise && fisher_in_gemm;
     for (long done = 0; done < nb; done += rows_per_pass) {
         const long n = nb - done < rows_per_pass ? nb - done : rows_per_pass;
-        int rc;
-        EventSet<3> evs;
-        cudaEvent_t *ev = evs.ev;
-        if (g_timing_on) {
-            CUDA_TRY(evs.create());
-            CUDA_TRY(cudaEventRecord(ev[0], st));
-        }
+        PassTimer timer(st);
+        int rc = timer.start();
+        if (rc) return rc;
         if (tiled)
             rc = launch_corr_mma(rows_op, cols_op, precision, E, T, V, V2, start + done, n, work, 4, 4,
                                   fisher_in_gemm ? S_eps : 0, st, t256, half16 ? 1 : 0);
@@ -3248,7 +3189,8 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
             rc = launch_corr_mma(rows_op, cols_op, precision, E, T, V, V2, start + done, n, work, (long)E * ld, ld,
                                   fisher_in_gemm ? S_eps : 0, st);
         if (rc) return rc;
-        if (g_timing_on) CUDA_TRY(cudaEventRecord(ev[1], st));
+        rc = timer.gemm_done();
+        if (rc) return rc;
         float *Kdst = sum_over_rows ? K : K + (size_t)done * E * E;
         const float beta = sum_over_rows ? 1.0f : 0.0f;
         if (tiled) {
@@ -3276,14 +3218,8 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
                 rc = launch_syrk_simt(work, n, E, V2, (long)E * ld, ld, beta, Kdst, sum_over_rows, st);
         }
         if (rc) return rc;
-        if (g_timing_on) {
-            CUDA_TRY(cudaEventRecord(ev[2], st));
-            CUDA_TRY(cudaEventSynchronize(ev[2]));
-            float a = 0.f, b = 0.f;
-            CUDA_TRY(cudaEventElapsedTime(&a, ev[0], ev[1]));
-            CUDA_TRY(cudaEventElapsedTime(&b, ev[1], ev[2]));
-            g_t_gemm += a, g_t_syrk += b, g_t_passes++;
-        }
+        rc = timer.end();
+        if (rc) return rc;
     }
     return FCMA_OK;
 }
@@ -3301,18 +3237,16 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
 // (E <= 32, power-of-two eps <= 32; fp32 or fp16 block), 0 = transposed block B + row pass
 static bool sym_uses_cols(int precision, int E, int eps, int flags)
 {
-    const char *f16i = diag_env("FCMA_F16_INTERMEDIATE");
-    bool half16 = (flags & FCMA_FLAG_F16_INTERMEDIATE) || precision == FCMA_PREC_BF16 || precision == FCMA_PREC_TF32;
-    if (f16i && (f16i[0] == '0' || f16i[0] == '1')) half16 = f16i[0] == '1';
-    const char *sc = diag_env("FCMA_SYM_COLS");
-    if ((sc && sc[0] == '0') || (flags & FCMA_FLAG_SYM_TRANSPOSED)) return false;
-    if (half16) {   // fp16 block: FCMA_SYM_COLS_F16=0 keeps the transposed copy + row pass (A/B)
-        const char *sh = diag_env("FCMA_SYM_COLS_F16");
-        if (sh && sh[0] == '0') return false;
-    }
+    if (flags & FCMA_FLAG_SYM_TRANSPOSED) return false;
     // 32 < E <= 64: the column kernel (fp32 block only) is opt-in; it halves the scratch per block row
-    if (E > 32 && (half16 || !(flags & FCMA_FLAG_COLS_WIDE))) return false;
+    if (E > 32 && (half_block(precision, flags) || !(flags & FCMA_FLAG_COLS_WIDE))) return false;
     return cols_supported(E, eps);
+}
+// scratch per block row of a symmetric pass over rows [start, V): block A needs E * round_up(V - start, 256) floats per
+// row; a transposed block B at most the same again
+static size_t sym_row_bytes(int precision, int E, int eps, int flags, long V, long start)
+{
+    return (sym_uses_cols(precision, E, eps, flags) ? 1 : 2) * fcma_work_bytes_per_row(E, V - start);
 }
 extern "C" int fcma_sym_uses_column_pass(int precision, int E, int eps, int flags)
 {
@@ -3345,16 +3279,12 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
     if (flags & FCMA_FLAG_FISHER_IN_PASS2) return fail(FCMA_EINVAL, "symmetric pipeline applies Fisher-z in the GEMM epilogue");
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
     const int S_eps = (E / eps) * eps;
-    // fp16 Fisher-z block: same rule as the plain pipeline (flag, or the single-product operand modes)
-    const char *f16i = diag_env("FCMA_F16_INTERMEDIATE");
-    bool half16 = (flags & FCMA_FLAG_F16_INTERMEDIATE) || precision == FCMA_PREC_BF16 || precision == FCMA_PREC_TF32;
-    if (f16i && (f16i[0] == '0' || f16i[0] == '1')) half16 = f16i[0] == '1';
+    const bool half16 = half_block(precision, flags);
     const size_t esz = half16 ? sizeof(__half) : sizeof(float);
     // column-direction pass (E <= 32; fp32 or fp16 block): the column voxels' sums are taken from block A itself, no
-    // transposed copy is stored.  FCMA_SYM_COLS=0 (fp16 block: FCMA_SYM_COLS_F16=0) keeps the transposed block B (A/B).
+    // transposed copy is stored.  FCMA_FLAG_SYM_TRANSPOSED keeps the transposed block B.
     const bool use_cols = sym_uses_cols(precision, E, eps, flags);
-    // per block row: A needs E * round_up(V - a, 256) floats; with a transposed block B at most the same again
-    const size_t row_bytes = (use_cols ? 1 : 2) * fcma_work_bytes_per_row(E, V - start);
+    const size_t row_bytes = sym_row_bytes(precision, E, eps, flags, V, start);
     // host-buffer mode with room for two blocks: the first TWO passes' GEMMs follow the upload group by group
     const bool grouped = hooks && hooks->ngroups > 0;
     const bool two = grouped && hooks->two_buffers && work_bytes / 2 / row_bytes >= 256;
@@ -3384,11 +3314,11 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
                                 e_begin, e_count, fixup);
     };
     // normalise + SYRK of one pass: rows of the block, then its columns (or the rows of the transposed copy)
-    auto syrk_pass = [&](const Pass &g, float *A, cudaEvent_t after_rows) -> int {
+    auto syrk_pass = [&](const Pass &g, float *A, PassTimer *timer) -> int {
         int rc = launch_norm_syrk(A, g.n, E, g.colsA, 256, 65536, eps, 1, mask_self ? 0 : -1, 1.0f, K + (size_t)g.a * E * E, 0,
                                   st, (long)E * 65536, half16 ? 1 : 0);
         if (rc) return rc;
-        if (after_rows) CUDA_TRY(cudaEventRecord(after_rows, st));
+        if (timer && (rc = timer->rows_done())) return rc;
         if (hooks && hooks->K_host) {
             // rows [a, a+n) of K are final now (the columns left of this pass arrived through earlier column passes)
             EventSet<1> rowdone;
@@ -3427,26 +3357,17 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
     }
     for (long p = first; p < npass; p++) {
         const Pass g = geometry(p);
-        EventSet<4> evs;
-        cudaEvent_t *ev = evs.ev;
-        if (g_timing_on) {
-            CUDA_TRY(evs.create());
-            CUDA_TRY(cudaEventRecord(ev[0], st));
-        }
-        int rc = gemm_pass(g, buf0, 0, E, true);
+        PassTimer timer(st);
+        int rc = timer.start();
         if (rc) return rc;
-        if (g_timing_on) CUDA_TRY(cudaEventRecord(ev[1], st));
-        rc = syrk_pass(g, buf0, g_timing_on ? ev[3] : nullptr);
+        rc = gemm_pass(g, buf0, 0, E, true);
         if (rc) return rc;
-        if (g_timing_on) {
-            CUDA_TRY(cudaEventRecord(ev[2], st));
-            CUDA_TRY(cudaEventSynchronize(ev[2]));
-            float x = 0.f, y = 0.f, z = 0.f;
-            CUDA_TRY(cudaEventElapsedTime(&x, ev[0], ev[1]));
-            CUDA_TRY(cudaEventElapsedTime(&y, ev[1], ev[2]));
-            CUDA_TRY(cudaEventElapsedTime(&z, ev[3], ev[2]));
-            g_t_gemm += x, g_t_syrk += y, g_t_syrk2 += z, g_t_passes++;
-        }
+        rc = timer.gemm_done();
+        if (rc) return rc;
+        rc = syrk_pass(g, buf0, &timer);
+        if (rc) return rc;
+        rc = timer.end();
+        if (rc) return rc;
     }
     return FCMA_OK;
 }
@@ -3468,7 +3389,7 @@ static int run_classifier_sym(const void *op, int precision, int E, int T, long 
     if (eps < 2 || !fused_supported(E, eps)) return fail(FCMA_EINVAL, "symmetric classifier kernel needs the fused path (E <= 64, power-of-two eps >= 2)");
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
     const int S_eps = (E / eps) * eps;
-    bool half16 = (flags & FCMA_FLAG_F16_INTERMEDIATE) || precision == FCMA_PREC_BF16 || precision == FCMA_PREC_TF32;
+    const bool half16 = half_block(precision, flags);
     const size_t esz = half16 ? sizeof(__half) : sizeof(float);
     const size_t row_bytes = fcma_work_bytes_per_row(E, V);
     const long rows_per_pass = (long)(work_bytes / row_bytes) & ~255L;
@@ -3482,14 +3403,13 @@ static int run_classifier_sym(const void *op, int precision, int E, int T, long 
         const long colsA = V - a, t256 = cdiv(colsA, 256), nt = cdiv(n, 256);
         if ((size_t)(nt * t256 * E) * 65536 * esz > work_bytes) return fail(FCMA_ENOMEM, "internal: symmetric pass does not fit the work buffer");
         SymOut so{nullptr};
-        EventSet<3> evs;
-        if (g_timing_on) {
-            CUDA_TRY(evs.create());
-            CUDA_TRY(cudaEventRecord(evs.ev[0], st));
-        }
-        int rc = launch_corr_mma(op, op, precision, E, T, V, V, a, n, work, 4, 4, S_eps, st, t256, half16 ? 1 : 0, &so);
+        PassTimer timer(st);
+        int rc = timer.start();
         if (rc) return rc;
-        if (g_timing_on) CUDA_TRY(cudaEventRecord(evs.ev[1], st));
+        rc = launch_corr_mma(op, op, precision, E, T, V, V, a, n, work, 4, 4, S_eps, st, t256, half16 ? 1 : 0, &so);
+        if (rc) return rc;
+        rc = timer.gemm_done();
+        if (rc) return rc;
         const long rb = t256 * (long)E * 65536;                       // elements between the 256-row blocks of the block
         const long sq = nt * 256 < colsA ? nt * 256 : colsA;          // columns of the diagonal square
         rc = launch_norm_syrk(work, n, E, sq, 256, 65536, eps, 1, mask_self ? 0 : -1, 1.0f, K, 1, st, (long)E * 65536,
@@ -3502,14 +3422,8 @@ static int run_classifier_sym(const void *op, int precision, int E, int T, long 
                                   half16 ? 1 : 0, rb, S + (size_t)E * E);
             if (rc) return rc;
         }
-        if (g_timing_on) {
-            CUDA_TRY(cudaEventRecord(evs.ev[2], st));
-            CUDA_TRY(cudaEventSynchronize(evs.ev[2]));
-            float x = 0.f, y = 0.f;
-            CUDA_TRY(cudaEventElapsedTime(&x, evs.ev[0], evs.ev[1]));
-            CUDA_TRY(cudaEventElapsedTime(&y, evs.ev[1], evs.ev[2]));
-            g_t_gemm += x, g_t_syrk += y, g_t_passes++;
-        }
+        rc = timer.end();
+        if (rc) return rc;
     }
     k_classifier_combine<<<(unsigned)cdiv((long)E * E, 256), 256, 0, st>>>(S, E * E, K);
     LAUNCH_CHECK("k_classifier_combine");
@@ -3526,7 +3440,7 @@ extern "C" int fcma_classifier_kernel_sym(const void *op, int precision, int E, 
 
 extern "C" long fcma_sym_rows_per_pass(int precision, int E, int eps, int flags, long V, long start, size_t work_bytes)
 {
-    const size_t row_bytes = (sym_uses_cols(precision, E, eps, flags) ? 1 : 2) * fcma_work_bytes_per_row(E, V - start);
+    const size_t row_bytes = sym_row_bytes(precision, E, eps, flags, V, start);
     return row_bytes ? (long)(work_bytes / row_bytes) & ~255L : 0;
 }
 
@@ -4337,18 +4251,12 @@ static int svm_cv_impl(const float *K_dev, long nv, int E, int nfolds, const voi
     const long nprob = nv * nfolds;
     if (shrinking) {
         const size_t smem = (size_t)4 * 64 * 64 * sizeof(float) + 4 * (4 * 64 * sizeof(double) + 2 * 64 * sizeof(int) + 64);
-        CUDA_TRY(cudaFuncSetAttribute(k_svm_cv_shrink, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_svm_cv_shrink<<<(unsigned)cdiv(nprob, 4), 128, smem, st>>>(K_dev, nv, E, nfolds, fd, C, tol, max_iter,
-                                                                    correct_dev, iters_dev, bits_dev);
-        LAUNCH_CHECK("k_svm_cv_shrink");
-        return FCMA_OK;
+        return launch_kernel(k_svm_cv_shrink, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv_shrink", K_dev, nv, E,
+                             nfolds, fd, C, tol, max_iter, correct_dev, iters_dev, bits_dev);
     }
     const size_t smem = (size_t)4 * 64 * 64 * sizeof(float);
-    CUDA_TRY(cudaFuncSetAttribute(k_svm_cv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_svm_cv<<<(unsigned)cdiv(nprob, 4), 128, smem, st>>>(K_dev, nv, E, nfolds, fd, C, tol, max_iter, correct_dev,
-                                                         iters_dev, bits_dev);
-    LAUNCH_CHECK("k_svm_cv");
-    return FCMA_OK;
+    return launch_kernel(k_svm_cv, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C, tol,
+                         max_iter, correct_dev, iters_dev, bits_dev);
 }
 
 // ---------------------------------------------------------------- host-buffer entry points
@@ -4489,7 +4397,7 @@ extern "C" int fcma_host_voxel_kernels_sym(const float *const *raw_host, const i
     const size_t opb = fcma_operand_bytes(precision, E, T, V);
     if (!opb) return fail(FCMA_EINVAL, "unknown precision %d", precision);
     const size_t ep_bytes = (size_t)E * T * V * sizeof(float), k_bytes = (size_t)V * E * E * sizeof(float);
-    const size_t per_row = (sym_uses_cols(precision, E, eps, flags) ? 1 : 2) * fcma_work_bytes_per_row(E, V);
+    const size_t per_row = sym_row_bytes(precision, E, eps, flags, V, 0);
     size_t freeb = 0, totalb = 0;
     CUDA_TRY(cudaMemGetInfo(&freeb, &totalb));
     {

@@ -11,9 +11,6 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from brainiak_b200 import _lib  # noqa: E402
-from brainiak_b200 import build as _build  # noqa: E402
-_build.build(diag=True)      # the FCMA_* knobs exist only in the diagnostic build (-DFCMA_DIAG)
-_lib.use_diag_build()
 from brainiak_b200.fcma import engine  # noqa: E402
 
 lib = _lib.load()
@@ -89,13 +86,12 @@ def big():
     del work
     torch.cuda.empty_cache()
     Ks = torch.empty((V, E, E), device=dev)
-    F16 = _lib.FLAG_F16_INTERMEDIATE
-    for name, rows, env, fl in (("sym fp32 block, column-direction pass over the block (default)", 2048, {}, 0),
-                                ("sym fp32 block, transposed copy B + row pass over it", 4096, {"FCMA_SYM_COLS": "0"}, 0),
-                                ("sym fp16 block, column pass", 2048, {}, F16),
-                                ("sym fp16 block, transposed copy B", 4096, {"FCMA_SYM_COLS_F16": "0"}, F16)):
+    F16, TR = _lib.FLAG_F16_INTERMEDIATE, _lib.FLAG_SYM_TRANSPOSED
+    for name, rows, fl in (("sym fp32 block, column-direction pass over the block (default)", 2048, 0),
+                           ("sym fp32 block, transposed copy B + row pass over it", 4096, TR),
+                           ("sym fp16 block, column pass", 2048, F16),
+                           ("sym fp16 block, transposed copy B", 4096, F16 | TR)):
         work = engine.SymWorkspace(E, V, rows, dev)
-        os.environ.update(env)
 
         def sym():
             Ks.zero_()
@@ -105,8 +101,6 @@ def big():
         d = (Ks - Kp).abs().max().item() / Kp.abs().max().item()
         print("%s: step %.1f ms (%.3g corr/s); gemm %.1f ms, syrk %.1f ms per step over %d passes; "
               "max|dK|/max|K| vs plain %.3g" % (name, ms, V * V * E / ms * 1e3, g, s, n, d), flush=True)
-        for k in env:
-            del os.environ[k]
         del work
         torch.cuda.empty_cache()
 
