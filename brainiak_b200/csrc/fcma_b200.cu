@@ -1114,6 +1114,90 @@ __global__ void __launch_bounds__(256) k_syrk_simt(const float *__restrict__ z, 
 // a6+a7 fused on warp MMAs: Fisher-z, within-subject z-score and K_i = Z_i Z_i^T in one pass
 // over the correlation block; the normalised values never leave registers.
 // ============================================================================================
+// z-score coefficients of a subject (two columns at once) from the sums of its EPS values and of their squares:
+// z = x * inv + mi.  nm = -mean, negvar = mean^2 - E[x^2] (both exact rescalings: EPS is a power of two); a variance
+// <= 0 gives inv = 0, so a constant subject normalises to zeros.
+template <int EPS>
+__device__ __forceinline__ void subject_coeffs(float2 msum, float2 s2sum, float2 &inv, float2 &mi)
+{
+    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
+    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
+    const float2 negvar = neg_variance<EPS>(nm, ns2);
+    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
+    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
+    mi = ffma2(nm, inv, splat2(0.f));
+}
+
+// Within-subject z-score of the values a lane holds in mma-fragment layout: epochs R*g + r (r < R) x NS slots x NU
+// columns, element v(r, s, u), two adjacent columns per packed fp32x2 op.  The epochs of one subject (EPS, a power of
+// two) lie inside the lane when EPS <= R, otherwise in EPS/R adjacent g-lanes (xor shuffles over lanes 4o).  Only
+// epochs of complete subjects (< S_eps) change.  The subject group is the outermost loop: moving it inside the
+// (slot, column) loops changes the kernels' instruction mix and spills.  all_valid (block-uniform, every real epoch in a
+// complete subject; padded epochs hold zeros and normalise to zeros) lets the shuffle path skip the per-lane select.
+template <int EPS, int R, int NS, int NU, typename V>
+__device__ __forceinline__ void zscore_frag(V &&v, int g, int S_eps, bool all_valid = false)
+{
+    auto apply = [&](int r, int s, int u, float2 inv, float2 mi) {
+        const float2 z = ffma2(make_float2(v(r, s, u), v(r, s, u + 1)), inv, mi);
+        v(r, s, u) = z.x, v(r, s, u + 1) = z.y;
+    };
+    if constexpr (EPS <= R) {
+#pragma unroll
+        for (int q = 0; q < R / EPS; q++) {
+            const bool valid = R * g + q * EPS < S_eps;
+#pragma unroll
+            for (int s = 0; s < NS; s++)
+#pragma unroll
+                for (int u = 0; u < NU; u += 2) {
+                    float2 m = splat2(0.f), s2 = splat2(0.f);
+#pragma unroll
+                    for (int b = 0; b < EPS; b++) {
+                        const float2 x = make_float2(v(q * EPS + b, s, u), v(q * EPS + b, s, u + 1));
+                        m = ffma2(x, splat2(1.f), m);
+                        s2 = ffma2(x, x, s2);
+                    }
+                    float2 inv, mi;
+                    subject_coeffs<EPS>(m, s2, inv, mi);
+                    if (valid) {
+#pragma unroll
+                        for (int b = 0; b < EPS; b++) apply(q * EPS + b, s, u, inv, mi);
+                    }
+                }
+        }
+    } else {
+        constexpr int L = EPS / R;   // adjacent g-lanes per subject
+        const bool valid = R * g < S_eps;
+#pragma unroll
+        for (int s = 0; s < NS; s++)
+#pragma unroll
+            for (int u = 0; u < NU; u += 2) {
+                float2 m = splat2(0.f), s2 = splat2(0.f);
+#pragma unroll
+                for (int r = 0; r < R; r++) {
+                    const float2 x = make_float2(v(r, s, u), v(r, s, u + 1));
+                    m = ffma2(x, splat2(1.f), m);
+                    s2 = ffma2(x, x, s2);
+                }
+#pragma unroll
+                for (int o = 1; o < L; o <<= 1) {
+                    m.x += __shfl_xor_sync(0xffffffffu, m.x, 4 * o);
+                    m.y += __shfl_xor_sync(0xffffffffu, m.y, 4 * o);
+                    s2.x += __shfl_xor_sync(0xffffffffu, s2.x, 4 * o);
+                    s2.y += __shfl_xor_sync(0xffffffffu, s2.y, 4 * o);
+                }
+                float2 inv, mi;
+                subject_coeffs<EPS>(m, s2, inv, mi);
+                if (all_valid) {   // uniform branch: no per-value select
+#pragma unroll
+                    for (int r = 0; r < R; r++) apply(r, s, u, inv, mi);
+                } else if (valid) {
+#pragma unroll
+                    for (int r = 0; r < R; r++) apply(r, s, u, inv, mi);
+                }
+            }
+    }
+}
+
 // One block (8 warps) per voxel row i; warps stride over 32-column chunks of the [E][n2] slab.
 // Lane (g = lane/4, t = lane%4) loads, as float4s, epochs R*g .. R*g+R-1 at columns
 // j0 + 16h + 4t .. +3 (h = 0,1).  These registers are at once
@@ -1128,13 +1212,7 @@ __global__ void __launch_bounds__(256) k_syrk_simt(const float *__restrict__ z, 
 // VEC: 0 scalar loads (unaligned fp32 block), 1 cp.async of an fp32 block, 2 cp.async of an fp16 block (tiled
 // intermediate written by the GEMM epilogue; a lane then takes 8 consecutive columns 8t..8t+7 per epoch as ONE
 // 16-byte copy -- which columns a k-slot stands for is irrelevant to a sum over columns).
-// F16_MMA: the z-scored values feed mma.m16n8k16 (fp16) instead of mma.m16n8k8 (tf32); compile-time switch kept for
-// A/B builds (-DFCMA_SYRK_TF32=1 restores the tf32 MMAs everywhere)
-#ifndef FCMA_SYRK_TF32
-constexpr bool F16_MMA = true;
-#else
-constexpr bool F16_MMA = false;
-#endif
+// EPS > 0: the z-scored values feed mma.m16n8k16 (fp16); EPS == 0 (already normalised input) keeps mma.m16n8k8 (tf32).
 template <int R, int EPS, bool FISHER, int VEC>
 __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
     k_norm_syrk(const float *__restrict__ C, long nb, int E, long n2, long stride_i, long ld, long chunk_step,
@@ -1338,85 +1416,8 @@ __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
                                 for (int u = 0; u < 4; u++) vals[r][h][u] = fisher_log2(vals[r][h][u]);
                         }
                 }
-                // ---- per (subject, column) mean / variance, two adjacent columns per packed fp32x2 op.
-                // nm = -mean, negvar = mean^2 - E[z^2] (both exact rescalings: EPS is a power of two)
-                auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
-                    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    mi = ffma2(nm, inv, splat2(0.f));
-                };
-                if constexpr (EPS <= R) {
-                    constexpr int G = EPS > 0 ? R / EPS : 1;
-#pragma unroll
-                    for (int q = 0; q < G; q++) {
-                        const bool valid = R * g + q * EPS < S_eps;
-#pragma unroll
-                        for (int h = 0; h < 2; h++)
-#pragma unroll
-                            for (int u = 0; u < 4; u += 2) {
-                                float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                                for (int b = 0; b < EPS; b++) {
-                                    const float2 x = make_float2(vals[q * EPS + b][h][u], vals[q * EPS + b][h][u + 1]);
-                                    m = ffma2(x, splat2(1.f), m);
-                                    s2 = ffma2(x, x, s2);
-                                }
-                                float2 inv, mi;
-                                finish(m, s2, inv, mi);
-                                if (valid) {
-#pragma unroll
-                                    for (int b = 0; b < EPS; b++) {
-                                        const float2 z = ffma2(
-                                            make_float2(vals[q * EPS + b][h][u], vals[q * EPS + b][h][u + 1]), inv, mi);
-                                        vals[q * EPS + b][h][u] = z.x, vals[q * EPS + b][h][u + 1] = z.y;
-                                    }
-                                }
-                            }
-                    }
-                } else {
-                    constexpr int L = EPS / R;  // adjacent g-lanes per subject
-                    // padded epochs (>= E) hold zeros and normalise to zeros, so when every real epoch belongs to a
-                    // complete subject no lane needs the select
-                    const bool all_valid = S_eps == E;   // block-uniform
-                    const bool valid = R * g < S_eps;
-#pragma unroll
-                    for (int h = 0; h < 2; h++)
-#pragma unroll
-                        for (int u = 0; u < 4; u += 2) {
-                            float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                            for (int r = 0; r < R; r++) {
-                                const float2 x = make_float2(vals[r][h][u], vals[r][h][u + 1]);
-                                m = ffma2(x, splat2(1.f), m);
-                                s2 = ffma2(x, x, s2);
-                            }
-#pragma unroll
-                            for (int o = 1; o < L; o <<= 1) {
-                                m.x += __shfl_xor_sync(0xffffffffu, m.x, 4 * o);
-                                m.y += __shfl_xor_sync(0xffffffffu, m.y, 4 * o);
-                                s2.x += __shfl_xor_sync(0xffffffffu, s2.x, 4 * o);
-                                s2.y += __shfl_xor_sync(0xffffffffu, s2.y, 4 * o);
-                            }
-                            float2 inv, mi;
-                            finish(m, s2, inv, mi);
-                            if (all_valid) {   // uniform branch: no per-value select
-#pragma unroll
-                                for (int r = 0; r < R; r++) {
-                                    const float2 z = ffma2(make_float2(vals[r][h][u], vals[r][h][u + 1]), inv, mi);
-                                    vals[r][h][u] = z.x, vals[r][h][u + 1] = z.y;
-                                }
-                            } else if (valid) {
-#pragma unroll
-                                for (int r = 0; r < R; r++) {
-                                    const float2 z = ffma2(make_float2(vals[r][h][u], vals[r][h][u + 1]), inv, mi);
-                                    vals[r][h][u] = z.x, vals[r][h][u + 1] = z.y;
-                                }
-                            }
-                        }
-                }
+                // ---- per (subject, column) z-score
+                zscore_frag<EPS, R, 2, 4>([&](int r, int h, int u) -> float & { return vals[r][h][u]; }, g, S_eps, S_eps == E);
             }
             // ---- self-correlation column mask (optional), tf32 rounding
             if (self_col >= j0 && self_col < j0 + 32) {  // warp-uniform, one chunk per row at most
@@ -1428,7 +1429,7 @@ __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
                         for (int u = 0; u < 4; u++)
                             if (j0 + (VEC == 2 ? 8 * t + 4 * h : 16 * h + 4 * t) + u == self_col) vals[r][h][u] = 0.f;
             }
-            if constexpr (EPS > 0 && F16_MMA) {
+            if constexpr (EPS > 0) {
                 // ---- K += Z Z^T with fp16 operands (m16n8k16): z-scored values are bounded by sqrt(EPS - 1) and the
                 // untouched trailing epochs hold |r| <= 1, so fp16 (11-bit significand like tf32, round to nearest
                 // even) loses nothing against the tf32 path below at half the MMA instructions and one pack per two
@@ -1576,6 +1577,127 @@ __global__ void __launch_bounds__(256, (R <= 4 ? 2 : 1))
 #endif
 constexpr int COLS_SEG_STEPS = FCMA_COLS_SEG_STEPS;   // 16-row steps between folds of the accumulators into K
 constexpr int COLS_BRICKS = 3;        // 64 KB bricks in flight / in use (cp.async pipeline depth)
+
+// One fold segment [seg0, seg1) of row steps through the cp.async brick ring: brick st+2 streams in while brick st is
+// used.  prefetch(st, slot) issues this thread's copies of row step st into ring slot `slot`; step(slot) consumes the
+// brick there.  Returns with every copy landed and every thread past its last read of the ring.
+template <typename Prefetch, typename Step>
+__device__ __forceinline__ void cols_ring_segment(long seg0, long seg1, Prefetch &&prefetch, Step &&step)
+{
+    static_assert(COLS_BRICKS == 3, "the ring holds the bricks st, st+1 and st+2");
+    int buf = 0;
+    prefetch(seg0, 0);
+    cp_async_commit();
+    if (seg0 + 1 < seg1) prefetch(seg0 + 1, 1);
+    cp_async_commit();
+    for (long st = seg0; st < seg1; st++) {
+        cp_async_wait<1>();        // brick `st` has landed (this thread's copies) ...
+        __syncthreads();           // ... and everybody's; every warp is also done with brick st-1,
+        if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);   // whose slot takes brick st+2
+        cp_async_commit();
+        step(buf);
+        buf = buf == COLS_BRICKS - 1 ? 0 : buf + 1;
+    }
+    cp_async_wait<0>();
+    __syncthreads();
+}
+
+// K += Z Z^T for one column on mma.m16n8k16 (fp16): h0[r] / h1[r] hold the z-scores of epoch slot r at k-slots
+// (2t, 2t+1) / (2t+8, 2t+9); every register is both an A and a B fragment
+template <int MT, int NT>
+__device__ __forceinline__ void mma_zzt(float (&acc)[MT][NT][4], const uint32_t (&h0)[NT], const uint32_t (&h1)[NT])
+{
+#pragma unroll
+    for (int mu = 0; mu < MT; mu++)
+#pragma unroll
+        for (int nu = 0; nu < NT; nu++)
+            mma_f16_16x8x16(acc[mu][nu], h0[2 * mu], h0[2 * mu + 1], h1[2 * mu], h1[2 * mu + 1], h0[nu], h1[nu]);
+}
+// the same from fp32 z-scores z(r, k) of epoch slot r and row slot k (k-slots 2t, 2t+1, 2t+8, 2t+9), rounded to fp16
+template <int MT, int NT, typename Z>
+__device__ __forceinline__ void mma_zzt(float (&acc)[MT][NT][4], Z &&z)
+{
+    uint32_t h0[NT], h1[NT];
+#pragma unroll
+    for (int r = 0; r < NT; r++) {
+        h0[r] = pack_half2_rn(z(r, 0), z(r, 1));
+        h1[r] = pack_half2_rn(z(r, 2), z(r, 3));
+    }
+    mma_zzt(acc, h0, h1);
+}
+
+// accumulators of mma_zzt with R = NT epochs per lane -> dst [EP][EP] in (epoch, epoch) order, EP = 8R: the lane's
+// rows are epochs R*g + 2mu (+1), its columns epochs R*2t + nu and R*(2t+1) + nu
+template <int MT, int NT>
+__device__ __forceinline__ void store_frag(float *dst, const float (&acc)[MT][NT][4], int g, int t)
+{
+    constexpr int R = NT, EP = 8 * R;
+#pragma unroll
+    for (int mu = 0; mu < MT; mu++)
+#pragma unroll
+        for (int nu = 0; nu < NT; nu++) {
+            const int row0 = R * g + 2 * mu, row1 = row0 + 1;
+            const int col0 = R * (2 * t) + nu, col1 = R * (2 * t + 1) + nu;
+            dst[row0 * EP + col0] = acc[mu][nu][0];
+            dst[row0 * EP + col1] = acc[mu][nu][1];
+            dst[row1 * EP + col0] = acc[mu][nu][2];
+            dst[row1 * EP + col1] = acc[mu][nu][3];
+        }
+}
+
+// K[col] += kernel of strip column col, col < ncols, for the strip's contiguous kernels at Kst: entry (a, b) is the
+// lower triangle of s_fold [col][EP*EP] mirrored (cython_blas.pyx:200-207).  The loop is latency-bound, so every thread
+// keeps 8 independent loads in flight, as 16-byte read-modify-writes when E*E % 4 == 0 and Kst is 16-byte aligned.
+// VEC / SCALAR: the paths a kernel compiles (only VEC: the caller guarantees the condition; only SCALAR: never vector).
+template <int EP, int NTHR, bool VEC = true, bool SCALAR = true>
+__device__ __forceinline__ void fold_strip(float *Kst, const float *s_fold, int E, int ncols)
+{
+    const int tid = threadIdx.x;
+    const int EE = E * E;
+    const int total = ncols * EE;
+    const bool vec = VEC && (!SCALAR || ((EE & 3) == 0 && (reinterpret_cast<uintptr_t>(Kst) & 15) == 0));
+    auto folded = [&](int idx) {
+        const int col = idx / EE, rem = idx - col * EE;
+        const int a = rem / E, b = rem - a * E;
+        const float *sk = s_fold + (size_t)col * (EP * EP);
+        return a >= b ? sk[a * EP + b] : sk[b * EP + a];
+    };
+    if (vec) {
+        float4 *K4 = reinterpret_cast<float4 *>(Kst);
+        const int total4 = total >> 2;
+        for (int base = tid; base < total4; base += NTHR * 8) {
+            float4 old[8];
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const int i4 = base + u * NTHR;
+                if (i4 < total4) old[u] = K4[i4];
+            }
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const int i4 = base + u * NTHR;
+                if (i4 < total4) {
+                    float4 o = old[u];
+                    o.x += folded(4 * i4), o.y += folded(4 * i4 + 1), o.z += folded(4 * i4 + 2), o.w += folded(4 * i4 + 3);
+                    K4[i4] = o;
+                }
+            }
+        }
+    } else {
+        for (int base = tid; base < total; base += NTHR * 8) {
+            float old[8];
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const int i1 = base + u * NTHR;
+                if (i1 < total) old[u] = Kst[i1];
+            }
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const int i1 = base + u * NTHR;
+                if (i1 < total) Kst[i1] = old[u] + folded(i1);
+            }
+        }
+    }
+}
 // CPW = columns per warp: 4 (8 warps, 4 accumulator sets, 255 registers) or 2 (16 warps, 2 accumulator sets, <= 128
 // registers: twice the warps to hide the dependent statistics / shuffle chains between the block barriers)
 // HALF: the block holds fp16 Fisher-z values (FCMA_FLAG_F16_INTERMEDIATE / single-product operand modes): a line
@@ -1650,6 +1772,9 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                     for (int b = 0; b < NT; b++)
 #pragma unroll
                         for (int d = 0; d < 4; d++) acc[c][a][b][d] = 0.f;
+            // the ring of cols_ring_segment, written out: this kernel runs at 255 registers, and with its step passed
+            // as a lambda ptxas rematerialises the fp32 brick's address arithmetic differently
+            static_assert(COLS_BRICKS == 3, "the ring holds the bricks st, st+1 and st+2");
             int buf = 0;
             prefetch(seg0, 0);
             cp_async_commit();
@@ -1658,7 +1783,7 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
             for (long st = seg0; st < seg1; st++) {
                 cp_async_wait<1>();        // brick `st` has landed (this thread's copies) ...
                 __syncthreads();           // ... and everybody's; every warp is also done with brick st-1,
-                if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);   // whose buffer takes brick st+2
+                if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);   // whose slot takes brick st+2
                 cp_async_commit();
                 // ---- this lane's 4 epochs x 4 rows x 4 columns
                 float vals[R][4][CPW];
@@ -1681,156 +1806,20 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                             vals[r][sl][0] = __uint_as_float(q.x), vals[r][sl][1] = __uint_as_float(q.y);
                         }
                     }
-                // ---- within-subject z-score per (row, column): statistics over the EPS epochs of a subject
-                auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
-                    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    mi = ffma2(nm, inv, splat2(0.f));
-                };
-                if constexpr (EPS <= R) {
-                    constexpr int G = R / EPS;
+                // ---- within-subject z-score per (row, column), then K_j += Z Z^T per column
+                zscore_frag<EPS, R, 4, CPW>([&](int r, int sl, int u) -> float & { return vals[r][sl][u]; }, g, S_eps);
 #pragma unroll
-                    for (int q = 0; q < G; q++) {
-                        const bool valid = R * g + q * EPS < S_eps;
-#pragma unroll
-                        for (int sl = 0; sl < 4; sl++)
-#pragma unroll
-                            for (int u = 0; u < CPW; u += 2) {
-                                float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                                for (int b = 0; b < EPS; b++) {
-                                    const float2 x = make_float2(vals[q * EPS + b][sl][u], vals[q * EPS + b][sl][u + 1]);
-                                    m = ffma2(x, splat2(1.f), m);
-                                    s2 = ffma2(x, x, s2);
-                                }
-                                float2 inv, mi;
-                                finish(m, s2, inv, mi);
-                                if (valid) {
-#pragma unroll
-                                    for (int b = 0; b < EPS; b++) {
-                                        const float2 z = ffma2(make_float2(vals[q * EPS + b][sl][u], vals[q * EPS + b][sl][u + 1]), inv, mi);
-                                        vals[q * EPS + b][sl][u] = z.x, vals[q * EPS + b][sl][u + 1] = z.y;
-                                    }
-                                }
-                            }
-                    }
-                } else {
-                    constexpr int L = EPS / R;   // adjacent g-lanes per subject
-                    const bool valid = R * g < S_eps;
-#pragma unroll
-                    for (int sl = 0; sl < 4; sl++)
-#pragma unroll
-                        for (int u = 0; u < CPW; u += 2) {
-                            float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                            for (int r = 0; r < R; r++) {
-                                const float2 x = make_float2(vals[r][sl][u], vals[r][sl][u + 1]);
-                                m = ffma2(x, splat2(1.f), m);
-                                s2 = ffma2(x, x, s2);
-                            }
-#pragma unroll
-                            for (int o = 1; o < L; o <<= 1) {
-                                m.x += __shfl_xor_sync(0xffffffffu, m.x, 4 * o);
-                                m.y += __shfl_xor_sync(0xffffffffu, m.y, 4 * o);
-                                s2.x += __shfl_xor_sync(0xffffffffu, s2.x, 4 * o);
-                                s2.y += __shfl_xor_sync(0xffffffffu, s2.y, 4 * o);
-                            }
-                            float2 inv, mi;
-                            finish(m, s2, inv, mi);
-                            if (valid) {
-#pragma unroll
-                                for (int r = 0; r < R; r++) {
-                                    const float2 z = ffma2(make_float2(vals[r][sl][u], vals[r][sl][u + 1]), inv, mi);
-                                    vals[r][sl][u] = z.x, vals[r][sl][u + 1] = z.y;
-                                }
-                            }
-                        }
-                }
-                // ---- K_j += Z Z^T: k-slots (2t, 2t+1) <-> row slots 0, 1 and (2t+8, 2t+9) <-> row slots 2, 3
-#pragma unroll
-                for (int c = 0; c < CPW; c++) {
-                    uint32_t h0[R], h1[R];
-#pragma unroll
-                    for (int r = 0; r < R; r++) {
-                        h0[r] = pack_half2_rn(vals[r][0][c], vals[r][1][c]);
-                        h1[r] = pack_half2_rn(vals[r][2][c], vals[r][3][c]);
-                    }
-#pragma unroll
-                    for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                        for (int nu = 0; nu < NT; nu++)
-                            mma_f16_16x8x16(acc[c][mu][nu], h0[2 * mu], h0[2 * mu + 1], h1[2 * mu], h1[2 * mu + 1], h0[nu], h1[nu]);
-                }
+                for (int c = 0; c < CPW; c++) mma_zzt(acc[c], [&](int r, int sl) { return vals[r][sl][c]; });
                 buf = buf == COLS_BRICKS - 1 ? 0 : buf + 1;
             }
-            // ---- fold the accumulators into K: registers -> smem [32 columns][EP*EP] -> mirrored, coalesced += on K
             cp_async_wait<0>();
             __syncthreads();
+            // ---- fold the accumulators into K: registers -> smem [32 columns][EP*EP] -> mirrored, coalesced += on K
 #pragma unroll
-            for (int c = 0; c < CPW; c++) {
-                float *dstk = s_fold + (size_t)(warp * CPW + c) * (EP * EP);
-#pragma unroll
-                for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                    for (int nu = 0; nu < NT; nu++) {
-                        const int row0 = R * g + 2 * mu, row1 = row0 + 1;
-                        const int col0 = R * (2 * t) + nu, col1 = R * (2 * t + 1) + nu;
-                        dstk[row0 * EP + col0] = acc[c][mu][nu][0];
-                        dstk[row0 * EP + col1] = acc[c][mu][nu][1];
-                        dstk[row1 * EP + col0] = acc[c][mu][nu][2];
-                        dstk[row1 * EP + col1] = acc[c][mu][nu][3];
-                    }
-            }
+            for (int c = 0; c < CPW; c++) store_frag(s_fold + (size_t)(warp * CPW + c) * (EP * EP), acc[c], g, t);
             __syncthreads();
-            const int EE = E * E;
             const long ncols = n2 - j0 < 32 ? n2 - j0 : 32;       // real columns of this strip
-            const int total = (int)ncols * EE;
-            float *Kst = K + (size_t)j0 * EE;                     // the strip's kernels are contiguous
-            auto folded = [&](int idx) {
-                const int col = idx / EE, rem = idx - col * EE;
-                const int a = rem / E, b = rem - a * E;
-                const float *sk = s_fold + (size_t)col * (EP * EP);
-                return a >= b ? sk[a * EP + b] : sk[b * EP + a];
-            };
-            if ((EE & 3) == 0 && ((reinterpret_cast<uintptr_t>(Kst) & 15) == 0)) {
-                // 16-byte read-modify-write, 8 independent loads in flight per thread (the loop is latency-bound)
-                float4 *K4 = reinterpret_cast<float4 *>(Kst);
-                const int total4 = total >> 2;
-                for (int base = tid; base < total4; base += NTHR * 8) {
-                    float4 old[8];
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i4 = base + u * NTHR;
-                        if (i4 < total4) old[u] = K4[i4];
-                    }
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i4 = base + u * NTHR;
-                        if (i4 < total4) {
-                            float4 o = old[u];
-                            o.x += folded(4 * i4), o.y += folded(4 * i4 + 1), o.z += folded(4 * i4 + 2), o.w += folded(4 * i4 + 3);
-                            K4[i4] = o;
-                        }
-                    }
-                }
-            } else {
-                for (int base = tid; base < total; base += NTHR * 8) {
-                    float old[8];
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i1 = base + u * NTHR;
-                        if (i1 < total) old[u] = Kst[i1];
-                    }
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i1 = base + u * NTHR;
-                        if (i1 < total) Kst[i1] = old[u] + folded(i1);
-                    }
-                }
-            }
+            fold_strip<EP, NTHR>(K + (size_t)j0 * (E * E), s_fold, E, (int)ncols);   // the strip's kernels are contiguous
             __syncthreads();
         }
     }
@@ -1842,12 +1831,12 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
 //
 // k_norm_syrk_cols above loads a brick straight into mma fragment layout (lane = (4 epochs, 4 rows)), so the statistics
 // of a subject are spread over lanes (shuffles), every value pair has to be re-paired for the packed fp32x2 FMAs
-// (15 % of its dynamic instructions are IMAD.MOV) and each lane repeats its partner's `finish`: ~680 warp
+// (15 % of its dynamic instructions are IMAD.MOV) and each lane repeats its partner's subject_coeffs: ~680 warp
 // instructions per warp and brick at two warps per scheduler.
 // Here warp w still owns columns 4w .. 4w+3 of the 32-column strip, but per brick [32 epochs][16 rows][32 columns]
 //   phase 1: lane l takes row (l & 15) and epochs 16*(l >> 4) .. +15: sixteen LDS.128 (4 adjacent columns of one
 //            (epoch, row) each), the subject statistics are plain in-thread sums over epochs on NATURAL fp32x2 pairs
-//            (columns 0|1 and 2|3) -- no shuffles (EPS = 32: one exchange with lane l ^ 16), one `finish` per (subject,
+//            (columns 0|1 and 2|3) -- no shuffles (EPS = 32: one exchange with lane l ^ 16), one subject_coeffs per (subject,
 //            column pair); the z-scored values are rounded to fp16 and stored as [column][row][32 epochs] (64 B per
 //            (column, row), 16-byte pieces swizzled with (row >> 1) & 3, bit 2 of the bank group from row & 1) into the
 //            warp's own 4 KB staging buffer;
@@ -1855,7 +1844,8 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
 //            the eight fragment registers that serve as A AND B operands of the eight mma.m16n8k16 of Z Z^T, with lane
 //            g <-> epoch 8*block + g: the accumulators are in NATURAL epoch order (no permutation to undo).
 // Only a __syncwarp separates the phases (a warp consumes what it staged).  The cp.async brick ring, the folds and the
-// arithmetic are those of k_norm_syrk_cols; the smem line swizzle is L & 7 (phase 1 reads 8 consecutive rows of one epoch).
+// arithmetic are shared with k_norm_syrk_cols (cols_ring_segment, subject_coeffs, mma_zzt; the fold is fold_strip's, written
+// out); the smem line swizzle is L & 7 (phase 1 reads 8 consecutive rows of one epoch).
 // ============================================================================================
 // CPW = 4: 8 warps x 4 columns (255 registers); CPW = 2: 16 warps x 2 columns (<= 128 registers, LDS.64): four warps per
 // scheduler instead of two
@@ -1921,16 +1911,7 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                     for (int b = 0; b < NT; b++)
 #pragma unroll
                         for (int d = 0; d < 4; d++) acc[c][a][b][d] = 0.f;
-            int buf = 0;
-            prefetch(seg0, 0);
-            cp_async_commit();
-            if (seg0 + 1 < seg1) prefetch(seg0 + 1, 1);
-            cp_async_commit();
-            for (long st = seg0; st < seg1; st++) {
-                cp_async_wait<1>();        // brick `st` has landed (this thread's copies) ...
-                __syncthreads();           // ... and everybody's; every warp is also done with brick st-1,
-                if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);   // whose buffer takes brick st+2
-                cp_async_commit();
+            cols_ring_segment(seg0, seg1, prefetch, [&](int buf) {
                 const uint32_t bb = brick0 + (uint32_t)buf * (uint32_t)BRICK + rd_base;
                 // ---- phase 1: 16 epochs x 4 columns of this lane's row, 8 epochs (one staged piece) at a time
                 float2 lo[16], hi[CPW == 4 ? 16 : 1];     // columns (0, 1) and (2, 3) of epoch 16*phalf + e
@@ -1945,14 +1926,6 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                         lo[e] = make_float2(__uint_as_float(q.x), __uint_as_float(q.y));
                     }
                 }
-                auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
-                    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    mi = ffma2(nm, inv, splat2(0.f));
-                };
                 constexpr int SPAN = EPS < 16 ? EPS : 16;          // epochs of one subject inside this lane
 #pragma unroll
                 for (int s0 = 0; s0 < 16; s0 += SPAN) {
@@ -1971,8 +1944,8 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                         }
                     }
                     float2 il, cl, ih = splat2(0.f), ch = splat2(0.f);
-                    finish(ml, ql, il, cl);
-                    if constexpr (CPW == 4) finish(mh, qh, ih, ch);
+                    subject_coeffs<EPS>(ml, ql, il, cl);
+                    if constexpr (CPW == 4) subject_coeffs<EPS>(mh, qh, ih, ch);
                     if (16 * phalf + s0 < S_eps) {       // epochs outside a complete subject stay as they are
 #pragma unroll
                         for (int e = s0; e < s0 + SPAN; e++) {
@@ -2004,19 +1977,12 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                     uint32_t h0[4], h1[4];      // epoch block r: rows (2t, 2t+1) / (2t+8, 2t+9) of epoch 8r + g
                     ldmatrix_x4_trans(lm_lo + (uint32_t)c * 1024u, h0[0], h0[1], h0[2], h0[3]);
                     ldmatrix_x4_trans(lm_hi + (uint32_t)c * 1024u, h1[0], h1[1], h1[2], h1[3]);
-#pragma unroll
-                    for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                        for (int nu = 0; nu < NT; nu++)
-                            mma_f16_16x8x16(acc[c][mu][nu], h0[2 * mu], h0[2 * mu + 1], h1[2 * mu], h1[2 * mu + 1], h0[nu], h1[nu]);
+                    mma_zzt(acc[c], h0, h1);
                 }
                 __syncwarp();      // the staging buffer is rewritten in the next step
-                buf = buf == COLS_BRICKS - 1 ? 0 : buf + 1;
-            }
+            });
             // ---- fold the accumulators into K: registers -> smem [32 columns][EP*EP] -> mirrored, coalesced += on K.
             // Natural epoch order: acc[c][mu][nu][{0,1}] = K[16 mu + g][8 nu + 2t + {0,1}], [{2,3}] = row 16 mu + g + 8.
-            cp_async_wait<0>();
-            __syncthreads();
 #pragma unroll
             for (int c = 0; c < CPW; c++) {
                 float *dstk = s_fold + (size_t)(warp * CPW + c) * (EP * EP);
@@ -2040,6 +2006,9 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                 const float *sk = s_fold + (size_t)col * (EP * EP);
                 return a >= b ? sk[a * EP + b] : sk[b * EP + a];
             };
+            // fold_strip, written out: at 16 warps x 128 registers (CPW = 2), calling the helper lets the compiler hoist
+            // the brick copies' address arithmetic out of the strip loop, which adds spills (52 -> 148 bytes of stores at
+            // EPS = 1) and ran 2.6 % slower (H100 80GB HBM3, 700 W limit)
             if ((EE & 3) == 0 && ((reinterpret_cast<uintptr_t>(Kst) & 15) == 0)) {
                 float4 *K4 = reinterpret_cast<float4 *>(Kst);
                 const int total4 = total >> 2;
@@ -2146,16 +2115,7 @@ __global__ void __launch_bounds__(256, 2)
                 for (int b = 0; b < NT; b++)
 #pragma unroll
                     for (int d = 0; d < 4; d++) acc[c][b][d] = 0.f;
-            int buf = 0;
-            prefetch(seg0, 0);
-            cp_async_commit();
-            if (seg0 + 1 < seg1) prefetch(seg0 + 1, 1);
-            cp_async_commit();
-            for (long st = seg0; st < seg1; st++) {
-                cp_async_wait<1>();
-                __syncthreads();
-                if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);
-                cp_async_commit();
+            cols_ring_segment(seg0, seg1, prefetch, [&](int buf) {
                 const uint32_t bb = brick0 + (uint32_t)buf * (uint32_t)BRICK + rd_base;
                 // ---- phase 1: 16 epochs x 2 columns of this lane's row
                 float2 v[16];
@@ -2169,13 +2129,8 @@ __global__ void __launch_bounds__(256, 2)
                     float2 m = splat2(0.f), q2 = splat2(0.f);
 #pragma unroll
                     for (int e = s0; e < s0 + EPS; e++) m = fadd2(m, v[e]), q2 = ffma2(v[e], v[e], q2);
-                    const float2 nm = ffma2(m, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(q2, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    float2 inv;
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    const float2 mi = ffma2(nm, inv, splat2(0.f));
+                    float2 inv, mi;
+                    subject_coeffs<EPS>(m, q2, inv, mi);
                     if (s0 < S_eps) {
 #pragma unroll
                         for (int e = s0; e < s0 + EPS; e++) v[e] = ffma2(v[e], inv, mi);
@@ -2202,11 +2157,8 @@ __global__ void __launch_bounds__(256, 2)
                         mma_f16_16x8x16(acc[c][nu], h00, h01, h10, h11, nu == 0 ? h00 : h01, nu == 0 ? h10 : h11);
                 }
                 __syncwarp();
-                buf = buf == COLS_BRICKS - 1 ? 0 : buf + 1;
-            }
+            });
             // ---- fold: acc[c][nu][{0,1}] = K[g][8 nu + 2t + {0,1}], [{2,3}] = row g + 8
-            cp_async_wait<0>();
-            __syncthreads();
 #pragma unroll
             for (int c = 0; c < CPW; c++) {
                 float *dstk = s_fold + (size_t)(warp * CPW + c) * (EP * EP);
@@ -2218,29 +2170,8 @@ __global__ void __launch_bounds__(256, 2)
                 }
             }
             __syncthreads();
-            const int EE = E * E;
             const long ncols = n2 - j0 < 32 ? n2 - j0 : 32;
-            const int total = (int)ncols * EE;
-            float *Kst = K + (size_t)j0 * EE;
-            auto folded = [&](int idx) {
-                const int col = idx / EE, rem = idx - col * EE;
-                const int a = rem / E, b = rem - a * E;
-                const float *sk = s_fold + (size_t)col * (EP * EP);
-                return a >= b ? sk[a * EP + b] : sk[b * EP + a];
-            };
-            for (int base = tid; base < total; base += NTHR * 8) {
-                float old[8];
-#pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int i1 = base + u * NTHR;
-                    if (i1 < total) old[u] = Kst[i1];
-                }
-#pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int i1 = base + u * NTHR;
-                    if (i1 < total) Kst[i1] = old[u] + folded(i1);
-                }
-            }
+            fold_strip<EP, NTHR, false>(K + (size_t)j0 * (E * E), s_fold, E, (int)ncols);
             __syncthreads();
         }
     }
@@ -2254,7 +2185,8 @@ __global__ void __launch_bounds__(256, 2)
 //     word(col, e, row) = col * 1092 + (e >> 3) * 136 + (e & 7) * 16 + row
 // (136: the eight epoch groups of a half warp's LDS.64 fall into distinct banks; 1092: the eight columns of a copying warp do),
 // so lane (g, t) of warp `col` reads its 8 epochs 8g .. 8g+7 x rows {2t, 2t+1}, {2t+8, 2t+9} with 16 conflict-free LDS.64.
-// Statistics, z-score, fragment roles and the fold are those of k_norm_syrk_cols with R = 8 epochs per lane.
+// Statistics, z-score, fragment roles and the fold are k_norm_syrk_cols's shared helpers (zscore_frag, mma_zzt, store_frag,
+// fold_strip) with R = 8 epochs per lane.
 // ============================================================================================
 template <int EPS>
 __global__ void __launch_bounds__(256, 1)
@@ -2313,16 +2245,7 @@ __global__ void __launch_bounds__(256, 1)
                 for (int b = 0; b < NT; b++)
 #pragma unroll
                     for (int d = 0; d < 4; d++) acc[a][b][d] = 0.f;
-            int buf = 0;
-            prefetch(seg0, 0);
-            cp_async_commit();
-            if (seg0 + 1 < seg1) prefetch(seg0 + 1, 1);
-            cp_async_commit();
-            for (long st = seg0; st < seg1; st++) {
-                cp_async_wait<1>();
-                __syncthreads();
-                if (st + 2 < seg1) prefetch(st + 2, buf == 0 ? 2 : buf - 1);
-                cp_async_commit();
+            cols_ring_segment(seg0, seg1, prefetch, [&](int buf) {
                 float2 lo[R], hi[R];     // rows (2t, 2t+1) and (2t+8, 2t+9) of epoch 8g + r, this warp's column
                 const uint32_t bb = brick0 + (uint32_t)buf * (uint32_t)BRICK + rd_base;
 #pragma unroll
@@ -2332,98 +2255,21 @@ __global__ void __launch_bounds__(256, 1)
                     lo[r] = make_float2(__uint_as_float(q0.x), __uint_as_float(q0.y));
                     hi[r] = make_float2(__uint_as_float(q1.x), __uint_as_float(q1.y));
                 }
-                auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
-                    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    mi = ffma2(nm, inv, splat2(0.f));
-                };
-                auto zscore = [&](float2 (&x)[R]) {
-                    if constexpr (EPS <= R) {
-                        constexpr int G = R / EPS;
-#pragma unroll
-                        for (int q = 0; q < G; q++) {
-                            float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                            for (int b = 0; b < EPS; b++) {
-                                m = ffma2(x[q * EPS + b], splat2(1.f), m);
-                                s2 = ffma2(x[q * EPS + b], x[q * EPS + b], s2);
-                            }
-                            float2 inv, mi;
-                            finish(m, s2, inv, mi);
-                            if (R * g + q * EPS < S_eps) {
-#pragma unroll
-                                for (int b = 0; b < EPS; b++) x[q * EPS + b] = ffma2(x[q * EPS + b], inv, mi);
-                            }
-                        }
-                    } else {
-                        constexpr int L = EPS / R;   // adjacent g-lanes per subject
-                        float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                        for (int r = 0; r < R; r++) {
-                            m = ffma2(x[r], splat2(1.f), m);
-                            s2 = ffma2(x[r], x[r], s2);
-                        }
-#pragma unroll
-                        for (int o = 1; o < L; o <<= 1) {
-                            m.x += __shfl_xor_sync(0xffffffffu, m.x, 4 * o);
-                            m.y += __shfl_xor_sync(0xffffffffu, m.y, 4 * o);
-                            s2.x += __shfl_xor_sync(0xffffffffu, s2.x, 4 * o);
-                            s2.y += __shfl_xor_sync(0xffffffffu, s2.y, 4 * o);
-                        }
-                        float2 inv, mi;
-                        finish(m, s2, inv, mi);
-                        if (R * g < S_eps) {
-#pragma unroll
-                            for (int r = 0; r < R; r++) x[r] = ffma2(x[r], inv, mi);
-                        }
-                    }
-                };
-                zscore(lo);
-                zscore(hi);
-                uint32_t h0[R], h1[R];
-#pragma unroll
-                for (int r = 0; r < R; r++) {
-                    h0[r] = pack_half2_rn(lo[r].x, lo[r].y);
-                    h1[r] = pack_half2_rn(hi[r].x, hi[r].y);
-                }
-#pragma unroll
-                for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                    for (int nu = 0; nu < NT; nu++)
-                        mma_f16_16x8x16(acc[mu][nu], h0[2 * mu], h0[2 * mu + 1], h1[2 * mu], h1[2 * mu + 1], h0[nu], h1[nu]);
-                buf = buf == COLS_BRICKS - 1 ? 0 : buf + 1;
-            }
+                // z-score: two row slots (the pair) per packed op, one column
+                zscore_frag<EPS, R, 1, 2>([&](int r, int, int u) -> float & { return u ? lo[r].y : lo[r].x; }, g, S_eps);
+                zscore_frag<EPS, R, 1, 2>([&](int r, int, int u) -> float & { return u ? hi[r].y : hi[r].x; }, g, S_eps);
+                mma_zzt(acc, [&](int r, int sl) {
+                    const float2 p = sl < 2 ? lo[r] : hi[r];
+                    return sl & 1 ? p.y : p.x;
+                });
+            });
             // ---- fold: registers -> smem [8 columns][64*64] -> mirrored, coalesced += on K
-            cp_async_wait<0>();
-            __syncthreads();
-            {
-                float *dstk = s_fold + (size_t)warp * (EP * EP);
-#pragma unroll
-                for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                    for (int nu = 0; nu < NT; nu++) {
-                        const int row0 = R * g + 2 * mu, row1 = row0 + 1;
-                        const int col0 = R * (2 * t) + nu, col1 = R * (2 * t + 1) + nu;
-                        dstk[row0 * EP + col0] = acc[mu][nu][0];
-                        dstk[row0 * EP + col1] = acc[mu][nu][1];
-                        dstk[row1 * EP + col0] = acc[mu][nu][2];
-                        dstk[row1 * EP + col1] = acc[mu][nu][3];
-                    }
-            }
+            store_frag(s_fold + (size_t)warp * (EP * EP), acc, g, t);
             __syncthreads();
             const int EE = E * E;
             const long ncols = n2 - j0 < 8 ? n2 - j0 : 8;
             const int total = (int)ncols * EE;
             float *Kst = K + (size_t)j0 * EE;
-            auto folded = [&](int idx) {
-                const int col = idx / EE, rem = idx - col * EE;
-                const int a = rem / E, b = rem - a * E;
-                const float *sk = s_fold + (size_t)col * (EP * EP);
-                return a >= b ? sk[a * EP + b] : sk[b * EP + a];
-            };
             if (E == 64 && ((reinterpret_cast<uintptr_t>(Kst) & 15) == 0)) {
                 // 16-byte read-modify-write, 8 independent loads in flight per thread; entry (a, b) of column `col`
                 float4 *K4 = reinterpret_cast<float4 *>(Kst);
@@ -2457,19 +2303,7 @@ __global__ void __launch_bounds__(256, 1)
                     }
                 }
             } else {
-                for (int base = tid; base < total; base += NTHR * 8) {
-                    float old[8];
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i1 = base + u * NTHR;
-                        if (i1 < total) old[u] = Kst[i1];
-                    }
-#pragma unroll
-                    for (int u = 0; u < 8; u++) {
-                        const int i1 = base + u * NTHR;
-                        if (i1 < total) Kst[i1] = old[u] + folded(i1);
-                    }
-                }
+                fold_strip<EP, NTHR, false>(Kst, s_fold, E, (int)ncols);
             }
             __syncthreads();
         }
@@ -2605,89 +2439,10 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
                                 for (int c = 0; c < CPW; c++) vals[r][sl][c] = 0.f;
                         }
                 }
-                // ---- within-subject z-score per (row, column): statistics over the EPS epochs of a subject
-                auto finish = [&](float2 msum, float2 s2sum, float2 &inv, float2 &mi) {
-                    const float2 nm = ffma2(msum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 ns2 = ffma2(s2sum, splat2(-1.0f / EPS), splat2(0.f));
-                    const float2 negvar = neg_variance<EPS>(nm, ns2);
-                    inv.x = negvar.x >= 0.f ? 0.f : rsqrt_ftz(-negvar.x);
-                    inv.y = negvar.y >= 0.f ? 0.f : rsqrt_ftz(-negvar.y);
-                    mi = ffma2(nm, inv, splat2(0.f));
-                };
-                if constexpr (EPS <= R) {
-                    constexpr int G = R / EPS;
+                // ---- within-subject z-score per (row, column), then K_j += Z Z^T per column
+                zscore_frag<EPS, R, 4, CPW>([&](int r, int sl, int u) -> float & { return vals[r][sl][u]; }, g, S_eps);
 #pragma unroll
-                    for (int q = 0; q < G; q++) {
-                        const bool valid = R * g + q * EPS < S_eps;
-#pragma unroll
-                        for (int sl = 0; sl < 4; sl++)
-#pragma unroll
-                            for (int u = 0; u < CPW; u += 2) {
-                                float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                                for (int b = 0; b < EPS; b++) {
-                                    const float2 x = make_float2(vals[q * EPS + b][sl][u], vals[q * EPS + b][sl][u + 1]);
-                                    m = ffma2(x, splat2(1.f), m);
-                                    s2 = ffma2(x, x, s2);
-                                }
-                                float2 inv, mi;
-                                finish(m, s2, inv, mi);
-                                if (valid) {
-#pragma unroll
-                                    for (int b = 0; b < EPS; b++) {
-                                        const float2 z = ffma2(make_float2(vals[q * EPS + b][sl][u], vals[q * EPS + b][sl][u + 1]), inv, mi);
-                                        vals[q * EPS + b][sl][u] = z.x, vals[q * EPS + b][sl][u + 1] = z.y;
-                                    }
-                                }
-                            }
-                    }
-                } else {
-                    constexpr int L = EPS / R;   // adjacent g-lanes per subject
-                    const bool valid = R * g < S_eps;
-#pragma unroll
-                    for (int sl = 0; sl < 4; sl++)
-#pragma unroll
-                        for (int u = 0; u < CPW; u += 2) {
-                            float2 m = splat2(0.f), s2 = splat2(0.f);
-#pragma unroll
-                            for (int r = 0; r < R; r++) {
-                                const float2 x = make_float2(vals[r][sl][u], vals[r][sl][u + 1]);
-                                m = ffma2(x, splat2(1.f), m);
-                                s2 = ffma2(x, x, s2);
-                            }
-#pragma unroll
-                            for (int o = 1; o < L; o <<= 1) {
-                                m.x += __shfl_xor_sync(0xffffffffu, m.x, 4 * o);
-                                m.y += __shfl_xor_sync(0xffffffffu, m.y, 4 * o);
-                                s2.x += __shfl_xor_sync(0xffffffffu, s2.x, 4 * o);
-                                s2.y += __shfl_xor_sync(0xffffffffu, s2.y, 4 * o);
-                            }
-                            float2 inv, mi;
-                            finish(m, s2, inv, mi);
-                            if (valid) {
-#pragma unroll
-                                for (int r = 0; r < R; r++) {
-                                    const float2 z = ffma2(make_float2(vals[r][sl][u], vals[r][sl][u + 1]), inv, mi);
-                                    vals[r][sl][u] = z.x, vals[r][sl][u + 1] = z.y;
-                                }
-                            }
-                        }
-                }
-                // ---- K_j += Z Z^T: k-slots (2t, 2t+1) <-> row slots 0, 1 and (2t+8, 2t+9) <-> row slots 2, 3
-#pragma unroll
-                for (int c = 0; c < CPW; c++) {
-                    uint32_t h0[R], h1[R];
-#pragma unroll
-                    for (int r = 0; r < R; r++) {
-                        h0[r] = pack_half2_rn(vals[r][0][c], vals[r][1][c]);
-                        h1[r] = pack_half2_rn(vals[r][2][c], vals[r][3][c]);
-                    }
-#pragma unroll
-                    for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                        for (int nu = 0; nu < NT; nu++)
-                            mma_f16_16x8x16(acc[c][mu][nu], h0[2 * mu], h0[2 * mu + 1], h1[2 * mu], h1[2 * mu + 1], h0[nu], h1[nu]);
-                }
+                for (int c = 0; c < CPW; c++) mma_zzt(acc[c], [&](int r, int sl) { return vals[r][sl][c]; });
                 it++;
                 if (++slot == COLS_BRICKS) slot = 0, par ^= 1u;
             }
@@ -2695,51 +2450,11 @@ __global__ void __launch_bounds__(32 * (32 / CPW), 1)
             // Every brick of the segment has been consumed (no bulk copy is in flight), all warps are past their reads.
             __syncthreads();
 #pragma unroll
-            for (int c = 0; c < CPW; c++) {
-                float *dstk = s_fold + (size_t)(warp * CPW + c) * (EP * EP);
-#pragma unroll
-                for (int mu = 0; mu < MT; mu++)
-#pragma unroll
-                    for (int nu = 0; nu < NT; nu++) {
-                        const int row0 = R * g + 2 * mu, row1 = row0 + 1;
-                        const int col0 = R * (2 * t) + nu, col1 = R * (2 * t + 1) + nu;
-                        dstk[row0 * EP + col0] = acc[c][mu][nu][0];
-                        dstk[row0 * EP + col1] = acc[c][mu][nu][1];
-                        dstk[row1 * EP + col0] = acc[c][mu][nu][2];
-                        dstk[row1 * EP + col1] = acc[c][mu][nu][3];
-                    }
-            }
+            for (int c = 0; c < CPW; c++) store_frag(s_fold + (size_t)(warp * CPW + c) * (EP * EP), acc[c], g, t);
             __syncthreads();
-            const int EE = E * E;
             const int ncols = n2 - j0 < 32 ? n2 - j0 : 32;       // real columns of this strip
-            const int total = ncols * EE;
-            float *Kst = K + (size_t)j0 * EE;                     // the strip's kernels are contiguous
-            auto folded = [&](int idx) {
-                const int col = idx / EE, rem = idx - col * EE;
-                const int a = rem / E, b = rem - a * E;
-                const float *sk = s_fold + (size_t)col * (EP * EP);
-                return a >= b ? sk[a * EP + b] : sk[b * EP + a];
-            };
-            // E % 4 == 0 here, and K + j0*E*E is 16-byte aligned whenever K is: 16-byte read-modify-write, 8 loads in flight
-            float4 *K4 = reinterpret_cast<float4 *>(Kst);
-            const int total4 = total >> 2;
-            for (int base = tid; base < total4; base += NTHR * 8) {
-                float4 old[8];
-#pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int i4 = base + u * NTHR;
-                    if (i4 < total4) old[u] = K4[i4];
-                }
-#pragma unroll
-                for (int u = 0; u < 8; u++) {
-                    const int i4 = base + u * NTHR;
-                    if (i4 < total4) {
-                        float4 o = old[u];
-                        o.x += folded(4 * i4), o.y += folded(4 * i4 + 1), o.z += folded(4 * i4 + 2), o.w += folded(4 * i4 + 3);
-                        K4[i4] = o;
-                    }
-                }
-            }
+            // E % 4 == 0 here, and K + j0*E*E is 16-byte aligned whenever K is: always 16-byte read-modify-writes
+            fold_strip<EP, NTHR, true, false>(K + (size_t)j0 * (E * E), s_fold, E, ncols);
             fence_proxy_async_smem();   // the fold's generic-proxy smem accesses are ordered before the next bulk copies
             __syncthreads();
         }
