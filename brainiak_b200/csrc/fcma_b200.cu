@@ -2685,6 +2685,9 @@ extern "C" int fcma_epoch_normalize(float *epochs_dev, int E, int T, long V, lon
     AsyncBuf te_buf;
     int *d_Te = nullptr;
     if (T_e) {
+        // a longer epoch would read (and overwrite) the next epoch's rows, or past the end for the last one
+        for (int e = 0; e < E; e++)
+            if (T_e[e] <= 0 || T_e[e] > T) return fail(FCMA_EINVAL, "epoch %d has length %d outside (0, %d]", e, T_e[e], T);
         CUDA_TRY(te_buf.alloc(sizeof(int) * E, st));
         d_Te = static_cast<int *>(te_buf.p);
         CUDA_TRY(cudaMemcpyAsync(d_Te, T_e, sizeof(int) * E, cudaMemcpyHostToDevice, st));
@@ -3267,24 +3270,32 @@ extern "C" int fcma_row_normalize(float *X_dev, long R, long D, long ld, int nan
 // ============================================================================================
 // Decimal shrink of voxelselector.py:409-412 / classifier.py:343-347, one warp per [E][E] kernel:
 //   nd = len(str(int(K[0][0]))); if nd > 2: K *= 10**(2-nd)   (float32 multiply, like numpy)
+// The digits of int(K00) are counted on the float itself, over its whole range (up to 39 digits): for an integer N,
+// trunc(|f|) >= N <=> |f| >= N, and for N = 10^k that holds exactly when |f| >= the smallest float32 >= 10^k (the table,
+// generated with Python integers and checked by tests/test_gpu_pack_and_side_kernels.py).  A negative value with
+// int() != 0 adds one for the '-' sign.  NaN and +-inf, where the reference's int() raises, give nd = 1: K untouched.
 __global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E, int *digits_out)
 {
+    constexpr float kPow10Ceil[38] = {
+        0x1.400000p+3f, 0x1.900000p+6f, 0x1.f40000p+9f, 0x1.388000p+13f, 0x1.86a000p+16f, 0x1.e84800p+19f,
+        0x1.312d00p+23f, 0x1.7d7840p+26f, 0x1.dcd650p+29f, 0x1.2a05f2p+33f, 0x1.748770p+36f, 0x1.d1a94cp+39f,
+        0x1.2309d0p+43f, 0x1.6bcc42p+46f, 0x1.c6bf54p+49f, 0x1.1c3794p+53f, 0x1.63457ap+56f, 0x1.bc16d8p+59f,
+        0x1.158e48p+63f, 0x1.5af1d8p+66f, 0x1.b1ae4ep+69f, 0x1.0f0cf2p+73f, 0x1.52d02ep+76f, 0x1.a78438p+79f,
+        0x1.08b2a4p+83f, 0x1.4adf4cp+86f, 0x1.9d9720p+89f, 0x1.027e74p+93f, 0x1.431e10p+96f, 0x1.93e594p+99f,
+        0x1.f8defap+102f, 0x1.3b8b5cp+106f, 0x1.8a6e34p+109f, 0x1.ed09c0p+112f, 0x1.342618p+116f, 0x1.812f9ep+119f,
+        0x1.e17b86p+122f, 0x1.2ced34p+126f,
+    };  // kPow10Ceil[k - 1] = smallest float32 >= 10^k
     const long v = (long)blockIdx.x * 4 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (v >= nv) return;
     float *Kv = K + (size_t)v * E * E;
     const float k00 = Kv[0];
     int nd = 1;
-    if (k00 == k00 && fabsf(k00) < 9.0e18f) {
-        long long iv = (long long)k00;  // int() truncates toward zero
-        if (iv < 0) {
-            nd = 2;                     // the '-' sign counts in len(str(.))
-            iv = -iv;
-        }
-        while (iv >= 10) {
-            iv /= 10;
-            nd++;
-        }
+    if (isfinite(k00)) {
+        const float a = fabsf(k00);
+#pragma unroll
+        for (int k = 0; k < 38; k++) nd += a >= kPow10Ceil[k];
+        if (k00 <= -1.0f) nd++;         // the '-' sign counts in len(str(.)); int(-0.5) is 0
     }
     if (digits_out && lane == 0) digits_out[v] = nd;
     if (nd > 2) {

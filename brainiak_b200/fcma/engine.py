@@ -454,9 +454,19 @@ def classifier_kernel(rows, cols, start, nb, eps, flags=0, work=None, out=None, 
     return out
 
 
+def _check_rows(x, name):
+    """The row kernels take float32 CUDA matrices with unit column stride and the row pitch ``stride(0)``."""
+    if x.dtype != torch.float32 or not x.is_cuda or x.dim() != 2 or x.stride(1) != 1:
+        raise ValueError("%s must be a 2-D float32 CUDA tensor with contiguous rows (stride(1) == 1)" % name)
+
+
 def gemm_nt(a, b):
     """``a @ b.T`` in fp32 FFMA (a12/a15)."""
     lib = _lib.load()
+    _check_rows(a, "a")
+    _check_rows(b, "b")
+    if a.shape[1] != b.shape[1] or a.device != b.device:
+        raise ValueError("gemm_nt: a and b must share their inner dimension and device")
     M, K = a.shape
     N = b.shape[0]
     out = torch.empty((M, N), dtype=torch.float32, device=a.device)
@@ -468,6 +478,7 @@ def gemm_nt(a, b):
 
 def row_normalize_(x, nan_to_zero=True):
     lib = _lib.load()
+    _check_rows(x, "x")
     R, D = x.shape
     with torch.cuda.device(x.device):
         _lib.check(lib.fcma_row_normalize(_ptr(x), R, D, x.stride(0), int(nan_to_zero), _stream_ptr()))
