@@ -71,6 +71,10 @@ SIGNATURES = {
                                         ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p]),
     "fcma_svm_cv_solve": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double, c_int, c_int,
                                   c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_svm_cv_solve_f64": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double,
+                                      c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_searchlight_kernels": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                         c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_gemm_nt": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_long, c_long, c_long, c_long,
                              c_long, c_void_p]),
     "fcma_row_normalize": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p]),

@@ -3399,10 +3399,16 @@ __device__ __forceinline__ void smo_pair_update(double &ai, double &aj, double y
     }
 }
 
-__global__ void __launch_bounds__(128) k_svm_cv(const float *__restrict__ K, long nv, int E, int nfolds,
+// Kernel element type KT: float (the FCMA kernels) or double (searchlight kernels).  Either way Q is float and QD, the
+// gradient and the decisions are double, as libsvm keeps them; an fp64 kernel therefore reproduces what libsvm computes
+// for a non-precomputed kernel (QD and the decision values from the double kernel function).  The double form reads the
+// decisions' kernel values from Kpred (the rbf difference form of k_function); the float form ignores Kpred.  Q is
+// formed as y_a y_b (float)K, which equals (float)(y_a y_b K) because y_a y_b = +-1 and rounding commutes with the sign.
+template <typename KT>
+__global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long nv, int E, int nfolds,
                                                const SvmFold *__restrict__ folds, double C, double eps, int max_iter,
                                                int *__restrict__ correct, int *__restrict__ iters,
-                                               unsigned long long *__restrict__ dec_bits)
+                                               unsigned long long *__restrict__ dec_bits, const KT *__restrict__ Kpred)
 {
     extern __shared__ float s_q[];   // [4 warps][nmax][nmax]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -3412,7 +3418,8 @@ __global__ void __launch_bounds__(128) k_svm_cv(const float *__restrict__ K, lon
     const int f = (int)(prob - v * nfolds);
     const SvmFold &fd = folds[f];
     const int n = fd.n_train;
-    const float *Kv = K + (size_t)v * E * E;
+    const KT *Kv = K + (size_t)v * E * E;
+    const KT *Kp = sizeof(KT) == 4 ? Kv : Kpred + (size_t)v * E * E;
     float *Q = s_q + (size_t)warp * 64 * 64;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
     const double TAU = 1e-12;
@@ -3436,7 +3443,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const float *__restrict__ K, lon
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
-            if (valid[s]) Q[a * 64 + k] = ya * (float)y[s] * Kv[(size_t)ia * E + idx[s]];
+            if (valid[s]) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + idx[s]];
         }
     }
     __syncwarp();
@@ -3565,7 +3572,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const float *__restrict__ K, lon
         double part = 0.0;
 #pragma unroll
         for (int s = 0; s < 2; s++)
-            if (valid[s] && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kv[(size_t)it * E + idx[s]];
+            if (valid[s] && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kp[(size_t)it * E + idx[s]];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
         const bool pred_pos = (part - rho) > 0;
@@ -3585,10 +3592,12 @@ __global__ void __launch_bounds__(128) k_svm_cv(const float *__restrict__ K, lon
 // index `pm` in the unpermuted sub-problem = active_set[]) travels between positions through a shared staging area when
 // do_shrinking swaps; Q stays in the unpermuted order and is addressed through pm.  Working-set selection, the G update
 // and rho run over [0, active); G_bar over all n.
-__global__ void __launch_bounds__(128) k_svm_cv_shrink(const float *__restrict__ K, long nv, int E, int nfolds,
+template <typename KT>
+__global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K, long nv, int E, int nfolds,
                                                       const SvmFold *__restrict__ folds, double C, double eps,
                                                       int max_iter, int *__restrict__ correct, int *__restrict__ iters,
-                                                      unsigned long long *__restrict__ dec_bits)
+                                                      unsigned long long *__restrict__ dec_bits,
+                                                      const KT *__restrict__ Kpred)
 {
     extern __shared__ float s_q[];   // [4 warps][64][64] Q, then per warp: 4 x 64 doubles, 2 x 64 ints, 64 bytes
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -3598,7 +3607,8 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const float *__restrict__
     const int f = (int)(prob - v * nfolds);
     const SvmFold &fd = folds[f];
     const int n = fd.n_train;
-    const float *Kv = K + (size_t)v * E * E;
+    const KT *Kv = K + (size_t)v * E * E;
+    const KT *Kp = sizeof(KT) == 4 ? Kv : Kpred + (size_t)v * E * E;
     float *Q = s_q + (size_t)warp * 64 * 64;
     double *stg_d = reinterpret_cast<double *>(s_q + 4 * 64 * 64) + warp * 4 * 64;
     int *stg_i = reinterpret_cast<int *>(reinterpret_cast<double *>(s_q + 4 * 64 * 64) + 4 * 4 * 64) + warp * 2 * 64;
@@ -3626,7 +3636,7 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const float *__restrict__
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
-            if (k < n) Q[a * 64 + k] = ya * (float)y[s] * Kv[(size_t)ia * E + fd.train_idx[k]];
+            if (k < n) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + fd.train_idx[k]];
         }
     }
     __syncwarp();
@@ -3905,7 +3915,7 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const float *__restrict__
         double part = 0.0;
 #pragma unroll
         for (int s = 0; s < 2; s++)
-            if ((lane + 32 * s) < n && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kv[(size_t)it * E + idx[s]];
+            if ((lane + 32 * s) < n && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kp[(size_t)it * E + idx[s]];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(FULL, part, off);
         const bool pred_pos = (part - rho) > 0;
@@ -3929,15 +3939,17 @@ extern "C" int fcma_shrink_kernels(float *K_dev, long nv, int E, int *digits_dev
     return FCMA_OK;
 }
 
-static int svm_cv_impl(const float *K_dev, long nv, int E, int nfolds, const void *folds_host, double C, double tol,
-                       int max_iter, int shrinking, int *correct_dev, int *iters_dev, unsigned long long *bits_dev,
-                       void *stream);
+template <typename KT>
+static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds, const void *folds_host, double C,
+                       double tol, int max_iter, int shrinking, int *correct_dev, int *iters_dev,
+                       unsigned long long *bits_dev, void *stream);
 extern "C" int fcma_svm_cv_precomputed(const float *K_dev, long nv, int E, int nfolds, const void *folds_host,
                                        double C, double tol, int max_iter, int *correct_dev, int *iters_dev,
                                        void *stream)
 {
     if (!correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_precomputed: null output");
-    return svm_cv_impl(K_dev, nv, E, nfolds, folds_host, C, tol, max_iter, 0, correct_dev, iters_dev, nullptr, stream);
+    return svm_cv_impl<float>(K_dev, nullptr, nv, E, nfolds, folds_host, C, tol, max_iter, 0, correct_dev, iters_dev,
+                              nullptr, stream);
 }
 // the general form: `shrinking` selects the restatement of libsvm's shrinking heuristic (scikit-learn's default); bits_dev
 // (optional) receives the binary DECISION of every held-out sample (bit t of bits_dev[v * nproblems + p]) -- the building
@@ -3947,12 +3959,24 @@ extern "C" int fcma_svm_cv_solve(const float *K_dev, long nv, int E, int nproble
                                  unsigned long long *bits_dev, int *iters_dev, void *stream)
 {
     if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve: no output requested");
-    return svm_cv_impl(K_dev, nv, E, nproblems, folds_host, C, tol, max_iter, shrinking, correct_dev, iters_dev, bits_dev,
-                       stream);
+    return svm_cv_impl<float>(K_dev, nullptr, nv, E, nproblems, folds_host, C, tol, max_iter, shrinking, correct_dev,
+                              iters_dev, bits_dev, stream);
 }
-static int svm_cv_impl(const float *K_dev, long nv, int E, int nfolds, const void *folds_host, double C, double tol,
-                       int max_iter, int shrinking, int *correct_dev, int *iters_dev, unsigned long long *bits_dev,
-                       void *stream)
+// the same solver on fp64 kernels: Q_ab = (float)(y_a y_b K_fit_ab), QD_a = K_fit_aa and the decisions
+// sum_k alpha_k y_k K_pred[t][k] - rho in double.  K_pred may be K_fit (linear kernel).
+extern "C" int fcma_svm_cv_solve_f64(const double *K_fit_dev, const double *K_pred_dev, long nv, int E, int nproblems,
+                                     const void *folds_host, double C, double tol, int max_iter, int shrinking,
+                                     int *correct_dev, unsigned long long *bits_dev, int *iters_dev, void *stream)
+{
+    if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64: no output requested");
+    if (!K_pred_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64: null K_pred");
+    return svm_cv_impl<double>(K_fit_dev, K_pred_dev, nv, E, nproblems, folds_host, C, tol, max_iter, shrinking,
+                               correct_dev, iters_dev, bits_dev, stream);
+}
+template <typename KT>
+static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds, const void *folds_host, double C,
+                       double tol, int max_iter, int shrinking, int *correct_dev, int *iters_dev,
+                       unsigned long long *bits_dev, void *stream)
 {
     int rc = check_device();
     if (rc) return rc;
@@ -3977,12 +4001,171 @@ static int svm_cv_impl(const float *K_dev, long nv, int E, int nfolds, const voi
     const long nprob = nv * nfolds;
     if (shrinking) {
         const size_t smem = (size_t)4 * 64 * 64 * sizeof(float) + 4 * (4 * 64 * sizeof(double) + 2 * 64 * sizeof(int) + 64);
-        return launch_kernel(k_svm_cv_shrink, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv_shrink", K_dev, nv, E,
-                             nfolds, fd, C, tol, max_iter, correct_dev, iters_dev, bits_dev);
+        return launch_kernel(k_svm_cv_shrink<KT>, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv_shrink", K_dev, nv,
+                             E, nfolds, fd, C, tol, max_iter, correct_dev, iters_dev, bits_dev, Kpred_dev);
     }
     const size_t smem = (size_t)4 * 64 * 64 * sizeof(float);
-    return launch_kernel(k_svm_cv, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C, tol,
-                         max_iter, correct_dev, iters_dev, bits_dev);
+    return launch_kernel(k_svm_cv<KT>, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C,
+                         tol, max_iter, correct_dev, iters_dev, bits_dev, Kpred_dev);
+}
+
+// ============================================================================================
+// Searchlight kernel matrices (MVPAVoxelSelector): for each centre c of a list, the [E][E] fp64 Gram matrix of the
+// centre's features -- the voxels of its (2r+1)^3 cube where mask and shape both hold, in C order of the cube -- with
+// the sample vectors x_e = vol[voxel][e] (volume [nx][ny][nz][E], epochs contiguous per voxel).
+//   kind 0 (linear): K_fit = G,  G_ab = sum_f x_a[f] x_b[f]
+//   kind 1 (rbf):    K_fit_ab  = exp(-gamma ((G_aa + G_bb) - 2 G_ab))   libsvm's kernel_rbf (x_square form, training)
+//                    K_pred_ab = exp(-gamma sum_f (x_a[f] - x_b[f])^2)   libsvm's k_function (difference form, decisions)
+// The products of float32 values are exact in fp64, so only the order of the additions (features in cube order, one
+// sequential sum per pair) can differ from the reference's BLAS dot; every operation is rounded separately (no FMA
+// contraction).  K_fit_aa is exactly 1 for rbf, as libsvm's QD.  One CTA per centre: the features' E-vectors are
+// staged through shared memory in chunks of SL_CHUNK cube positions (any radius), each thread owns up to SL_PAIRS
+// pairs a <= b of the upper triangle, and the finished matrix goes out through shared memory in coalesced rows.
+#define SL_THREADS 256
+#define SL_CHUNK 32
+#define SL_PAIRS 9   // ceil(64 * 65 / 2 / SL_THREADS)
+
+template <int KIND>
+__global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float *__restrict__ vol, int ny, int nz, int E,
+                                                                    const unsigned char *__restrict__ mask, int r,
+                                                                    const unsigned char *__restrict__ shape,
+                                                                    const long *__restrict__ centres,
+                                                                    const double *__restrict__ gamma,
+                                                                    double *__restrict__ K_fit, double *__restrict__ K_pred)
+{
+    extern __shared__ double s_sl[];
+    double *tile = s_sl;                                                   // [E][E]
+    double *diag = tile + E * E;                                           // [E] G_aa
+    float *xs = reinterpret_cast<float *>(diag + E);                       // [SL_CHUNK][E]
+    unsigned char *act = reinterpret_cast<unsigned char *>(xs + SL_CHUNK * E);   // [SL_CHUNK]
+    const int tid = threadIdx.x;
+    const long m = blockIdx.x;
+    const long c = centres[m];
+    const int cz = (int)(c % nz), cy = (int)((c / nz) % ny), cx = (int)(c / ((long)nz * ny));
+    const int side = 2 * r + 1, ncube = side * side * side;
+    const int P = E * (E + 1) / 2;
+
+    int pa[SL_PAIRS], pb[SL_PAIRS];
+    double g[SL_PAIRS], d[SL_PAIRS];
+#pragma unroll
+    for (int s = 0; s < SL_PAIRS; s++) {
+        const int p = tid + s * SL_THREADS;
+        int a = 0, rem = p;
+        // row a of the upper triangle holds the E - a pairs (a, a..E-1)
+        while (p < P && rem >= E - a) rem -= E - a++;
+        pa[s] = p < P ? a : -1;
+        pb[s] = p < P ? a + rem : -1;
+        g[s] = 0.0;
+        d[s] = 0.0;
+    }
+
+    for (int o0 = 0; o0 < ncube; o0 += SL_CHUNK) {
+        const int nch = min(SL_CHUNK, ncube - o0);
+        __syncthreads();
+        if (tid < nch) {
+            const int o = o0 + tid;
+            const int i = o / (side * side), j = (o / side) % side, k = o % side;
+            const long vox = ((long)(cx - r + i) * ny + (cy - r + j)) * nz + (cz - r + k);
+            act[tid] = shape[o] && mask[vox];
+        }
+        __syncthreads();
+        for (int idx = tid; idx < nch * E; idx += SL_THREADS) {
+            const int q = idx / E, e = idx - q * E;
+            if (act[q]) {
+                const int o = o0 + q;
+                const int i = o / (side * side), j = (o / side) % side, k = o % side;
+                const long vox = ((long)(cx - r + i) * ny + (cy - r + j)) * nz + (cz - r + k);
+                xs[q * E + e] = vol[vox * E + e];
+            }
+        }
+        __syncthreads();
+        for (int q = 0; q < nch; q++) {
+            if (!act[q]) continue;
+            const float *xq = xs + q * E;
+#pragma unroll
+            for (int s = 0; s < SL_PAIRS; s++) {
+                if (pa[s] < 0) continue;
+                const double xa = (double)xq[pa[s]], xb = (double)xq[pb[s]];
+                g[s] = __dadd_rn(g[s], __dmul_rn(xa, xb));
+                if (KIND == 1) {
+                    const double df = __dsub_rn(xa, xb);
+                    d[s] = __dadd_rn(d[s], __dmul_rn(df, df));
+                }
+            }
+        }
+    }
+
+    const size_t base = (size_t)m * E * E;
+    if (KIND == 1) {
+#pragma unroll
+        for (int s = 0; s < SL_PAIRS; s++)
+            if (pa[s] >= 0 && pa[s] == pb[s]) diag[pa[s]] = g[s];
+    }
+    __syncthreads();
+    const double gm = KIND == 1 ? gamma[m] : 0.0;
+#pragma unroll
+    for (int s = 0; s < SL_PAIRS; s++) {
+        if (pa[s] < 0) continue;
+        double v = g[s];
+        if (KIND == 1) v = exp(__dmul_rn(-gm, __dsub_rn(__dadd_rn(diag[pa[s]], diag[pb[s]]), __dmul_rn(2.0, g[s]))));
+        tile[pa[s] * E + pb[s]] = v;
+        tile[pb[s] * E + pa[s]] = v;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < E * E; idx += SL_THREADS) K_fit[base + idx] = tile[idx];
+    if (KIND == 1) {
+        __syncthreads();
+#pragma unroll
+        for (int s = 0; s < SL_PAIRS; s++) {
+            if (pa[s] < 0) continue;
+            const double v = exp(__dmul_rn(-gm, d[s]));
+            tile[pa[s] * E + pb[s]] = v;
+            tile[pb[s] * E + pa[s]] = v;
+        }
+        __syncthreads();
+        for (int idx = tid; idx < E * E; idx += SL_THREADS) K_pred[base + idx] = tile[idx];
+    }
+}
+
+extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E,
+                                        const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
+                                        const long *centres_host, long M, int kind, const double *gamma_host,
+                                        double *K_fit_dev, double *K_pred_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (!vol_dev || !mask_dev || !shape_dev || !centres_host || !K_fit_dev || M <= 0 || nx <= 0 || ny <= 0 || nz <= 0)
+        return fail(FCMA_EINVAL, "fcma_searchlight_kernels: null buffer or empty volume / centre list");
+    if (E < 1 || E > 64) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: E = %d outside 1..64", E);
+    if (sl_rad < 0) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: negative sl_rad");
+    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: kind must be 0 (linear) or 1 (rbf)");
+    if (kind == 1 && (!gamma_host || !K_pred_dev))
+        return fail(FCMA_EINVAL, "fcma_searchlight_kernels: rbf needs gamma and K_pred");
+    if (M > 0x7fffffffL) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: too many centres in one call");
+    for (long m = 0; m < M; m++) {
+        const long c = centres_host[m];
+        if (c < 0 || c >= nx * ny * nz) return fail(FCMA_EINVAL, "centre %ld: index %ld outside the volume", m, c);
+        const long z = c % nz, y = (c / nz) % ny, x = c / (nz * ny);
+        if (x < sl_rad || y < sl_rad || z < sl_rad || x >= nx - sl_rad || y >= ny - sl_rad || z >= nz - sl_rad)
+            return fail(FCMA_EINVAL, "centre %ld (%ld, %ld, %ld) is closer than sl_rad = %d to a face", m, x, y, z, sl_rad);
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    AsyncBuf cbuf, gbuf;
+    CUDA_TRY(cbuf.alloc(sizeof(long) * M, st));
+    CUDA_TRY(cudaMemcpyAsync(cbuf.p, centres_host, sizeof(long) * M, cudaMemcpyHostToDevice, st));
+    if (kind == 1) {
+        CUDA_TRY(gbuf.alloc(sizeof(double) * M, st));
+        CUDA_TRY(cudaMemcpyAsync(gbuf.p, gamma_host, sizeof(double) * M, cudaMemcpyHostToDevice, st));
+    }
+    const size_t smem = (size_t)E * E * sizeof(double) + E * sizeof(double) + SL_CHUNK * E * sizeof(float) + SL_CHUNK;
+    const long *cdev = static_cast<const long *>(cbuf.p);
+    const double *gdev = static_cast<const double *>(gbuf.p);
+    if (kind == 0)
+        return launch_kernel(k_searchlight_kernels<0>, (unsigned)M, SL_THREADS, smem, st, "k_searchlight_kernels",
+                             vol_dev, (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev,
+                             K_pred_dev);
+    return launch_kernel(k_searchlight_kernels<1>, (unsigned)M, SL_THREADS, smem, st, "k_searchlight_kernels", vol_dev,
+                         (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev, K_pred_dev);
 }
 
 // ---------------------------------------------------------------- host-buffer entry points

@@ -690,3 +690,113 @@ def svm_cv_precomputed(K, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, folds
     scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]   # accuracy_score per fold
     acc = scores.mean(axis=1)                                                   # cross_val_score(...).mean()
     return (acc, iters.cpu().numpy()) if return_iters else acc
+
+
+def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, shrinking=True, folds=None,
+               return_iters=False):
+    """``svm_cv_precomputed`` on fp64 kernels: ``K_fit`` / ``K_pred`` float64 CUDA ``[nv, E, E]`` (``K_pred`` may be
+    ``K_fit``).  The solver keeps Q in float and QD, the gradient and the decisions in double with QD and the decisions
+    read from the double kernels, which is what libsvm computes for ``SVC(kernel='linear' | 'rbf')`` on features whose
+    fp64 kernel values these are (see k_searchlight_kernels)."""
+    lib = _lib.load()
+    if K_fit.dtype != torch.float64 or K_pred.dtype != torch.float64 or K_fit.shape != K_pred.shape \
+            or K_fit.dim() != 3 or K_fit.shape[1] != K_fit.shape[2]:
+        raise ValueError("K_fit and K_pred must be float64 [nv, E, E] of the same shape")
+    if not (K_fit.is_contiguous() and K_pred.is_contiguous()):
+        raise ValueError("K_fit and K_pred must be contiguous")
+    nv, E, _ = K_fit.shape
+    if folds is None:
+        folds = make_svm_folds(labels, num_folds)
+    nprob = folds.nproblems
+    cap = int(max_iter if max_iter and max_iter > 0 else 10000000)
+    two = len(folds.classes) == 2
+    with torch.cuda.device(K_fit.device):
+        iters = torch.empty((nv, nprob), dtype=torch.int32, device=K_fit.device) if return_iters else None
+        correct = torch.empty((nv, nprob), dtype=torch.int32, device=K_fit.device) if two else None
+        bits = None if two else torch.empty((nv, nprob), dtype=torch.int64, device=K_fit.device)
+        _lib.check(lib.fcma_svm_cv_solve_f64(_ptr(K_fit), _ptr(K_pred), nv, E, nprob,
+                                             ctypes.cast(folds.structs, ctypes.c_void_p), float(C), float(tol), cap,
+                                             1 if shrinking else 0, _ptr(correct) if two else None,
+                                             _ptr(bits) if not two else None,
+                                             _ptr(iters) if iters is not None else None, _stream_ptr()))
+        if not two:
+            correct = _ovo_vote(bits, folds)
+    scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]
+    acc = scores.mean(axis=1)
+    return (acc, iters.cpu().numpy()) if return_iters else acc
+
+
+# ------------------------------------------------------------------ searchlight (MVPAVoxelSelector)
+def searchlight_centres(mask, sl_rad, shape, min_active=0):
+    """Centres of the reference's searchlight (searchlight.py:542-578) over a 3-D ``mask``: the mask voxels at least
+    ``sl_rad`` from every face whose cube satisfies ``count(mask & shape) / cube.size > min_active`` (no test when
+    ``min_active == 0``).  Returns ``(centres, n_features)``: int64 linear indices into ``mask`` in C order, and the
+    number of features (voxels of ``mask & shape`` in the cube) of each."""
+    from scipy import ndimage
+    mask = np.asarray(mask).astype(bool)
+    shape = np.asarray(shape).astype(bool)
+    r = int(sl_rad)
+    if mask.ndim != 3 or shape.shape != (2 * r + 1,) * 3:
+        raise ValueError("mask must be 3-D and shape (2*sl_rad+1)^3")
+    # counts[c] = sum_o mask[c - r + o] * shape[o]: an integer correlation centred on the cube
+    counts = ndimage.correlate(mask.astype(np.int32), shape.astype(np.int32), mode="constant", cval=0)
+    inner = np.zeros_like(mask)
+    if all(n > 2 * r for n in mask.shape):
+        inner[tuple(slice(r, n - r) for n in mask.shape)] = True
+    sel = mask & inner
+    if min_active != 0:
+        sel &= (counts / shape.size) > min_active
+    centres = np.flatnonzero(sel).astype(np.int64)
+    return centres, counts.ravel()[centres].astype(np.int64)
+
+
+def searchlight_used_voxels(mask, centres, sl_rad, shape):
+    """Boolean volume of the voxels that are a feature of at least one of ``centres``."""
+    from scipy import ndimage
+    mask = np.asarray(mask).astype(bool)
+    ind = np.zeros(mask.size, dtype=np.int32)
+    ind[np.asarray(centres, dtype=np.int64)] = 1
+    # used[v] = sum_o ind[v + r - o] * shape[o]  (v = c - r + o)
+    cover = ndimage.convolve(ind.reshape(mask.shape), np.asarray(shape).astype(np.int32), mode="constant", cval=0)
+    return mask & (cover > 0)
+
+
+def searchlight_kernels(vol, mask, sl_rad, shape, centres, kind="linear", gamma=None):
+    """fp64 kernel matrices of searchlight centres (k_searchlight_kernels): ``vol`` float32 CUDA ``[X, Y, Z, E]``,
+    ``mask`` / ``shape`` uint8 (or bool) CUDA volumes, ``centres`` int64 host indices (``searchlight_centres``).
+    ``kind='linear'``: returns ``(G, G)``; ``kind='rbf'`` with one ``gamma`` per centre: ``(K_fit, K_pred)``, the
+    x_square form libsvm trains with and the difference form its decisions use.  Both float64 ``[M, E, E]``."""
+    lib = _lib.load()
+    if vol.dim() != 4 or vol.dtype != torch.float32 or not vol.is_contiguous():
+        raise ValueError("vol must be a contiguous float32 [X, Y, Z, E] tensor")
+    X, Y, Z, E = vol.shape
+    if tuple(mask.shape) != (X, Y, Z):
+        raise ValueError("mask shape %s does not match the volume %s" % (tuple(mask.shape), (X, Y, Z)))
+    side = 2 * int(sl_rad) + 1
+    if tuple(shape.shape) != (side, side, side):
+        raise ValueError("shape must be (2*sl_rad+1)^3")
+    mask = mask.to(device=vol.device, dtype=torch.uint8).contiguous()
+    shape = shape.to(device=vol.device, dtype=torch.uint8).contiguous()
+    c = np.ascontiguousarray(centres, dtype=np.int64)
+    M = len(c)
+    if kind not in ("linear", "rbf"):
+        raise ValueError("kind must be 'linear' or 'rbf', not %r" % (kind,))
+    kcode = 0 if kind == "linear" else 1
+    g = None
+    if kcode == 1:
+        if gamma is None:
+            raise ValueError("kind='rbf' needs gamma (a number or one per centre)")
+        g = np.asarray(gamma, dtype=np.float64)
+        if g.ndim > 1 or (g.ndim == 1 and len(g) != M):
+            raise ValueError("gamma must be a number or one value per centre (%d)" % M)
+        if not (np.isfinite(g).all() and (g >= 0).all()):
+            raise ValueError("gamma must be finite and non-negative")
+        g = np.ascontiguousarray(np.broadcast_to(g, (M,)))
+    K_fit = torch.empty((M, E, E), dtype=torch.float64, device=vol.device)
+    K_pred = K_fit if kcode == 0 else torch.empty_like(K_fit)
+    with torch.cuda.device(vol.device):
+        _lib.check(lib.fcma_searchlight_kernels(_ptr(vol), X, Y, Z, E, _ptr(mask), int(sl_rad), _ptr(shape),
+                                                c.ctypes.data_as(ctypes.c_void_p), M, kcode,
+                                                g.ctypes.data_as(ctypes.c_void_p) if g is not None else None,
+                                                _ptr(K_fit), _ptr(K_pred) if kcode == 1 else None, _stream_ptr()))
+    return K_fit, K_pred

@@ -1,17 +1,28 @@
-"""Epoch separation + the per-epoch normalisation (the "normalise prologue") on the GPU.
+"""Epoch separation + the per-epoch normalisation (the "normalise prologue") on the GPU, and the host-side epoch
+averaging of the activity-based (MVPA) path.
 
 Mirrors the arithmetic of ``brainiak.fcma.preprocessing._separate_epochs`` (reference
 preprocessing.py:41-92).  NIfTI loading / masking (preprocessing.py:156-232 via brainiak.image) is
-out of scope: the functions here take the already masked ``[nVoxels, nTRs]`` activity arrays.
+out of scope: the functions here take the already masked ``[nVoxels, nTRs]`` activity arrays, or images that
+yield their data through ``get_fdata()``, or plain arrays.
+
+``generate_epochs_info``, ``prepare_mvpa_data`` and ``prepare_searchlight_mvpa_data`` (reference
+preprocessing.py:235-414) average each epoch and z-score within subject.  They are not a hot path and run on the host
+with the reference's numpy / scipy operations, so their output is bit-identical to the reference's.
 """
+import logging
 from enum import Enum
 
 import numpy as np
+from scipy.stats.mstats import zscore
 
 from .. import _lib
 from . import engine
 
-__all__ = ["separate_epochs", "separate_epochs_device", "broadcast_epochs", "prepare_fcma_data", "RandomType"]
+__all__ = ["separate_epochs", "separate_epochs_device", "broadcast_epochs", "prepare_fcma_data", "RandomType",
+           "generate_epochs_info", "prepare_mvpa_data", "prepare_searchlight_mvpa_data"]
+
+logger = logging.getLogger(__name__)
 
 
 def _epoch_slices(activity_data, epoch_list):
@@ -145,3 +156,91 @@ def prepare_fcma_data(images, conditions, mask1, mask2=None, random=RandomType.N
         host = ep.cpu().numpy()
         out.append([np.ascontiguousarray(host[e, :T_e[e], :]) for e in range(len(T_e))])
     return out[0], (out[1] if len(out) > 1 else None), labels
+
+
+# ------------------------------------------------------------------ activity-based (MVPA) preprocessing, on the host
+def generate_epochs_info(epoch_list):
+    """Epochs of ``epoch_list`` (one ``[condition, nEpochs, nTRs]`` 0/1 array per subject, every epoch a contiguous run
+    of TRs) as a list of ``(label, sid, start, end)``, ``end`` exclusive, in the reference's order: subject, then
+    condition, then epoch (preprocessing.py:235-271)."""
+    epoch_info = []
+    for sid, epoch in enumerate(epoch_list):
+        for cond in range(epoch.shape[0]):
+            sub_epoch = epoch[cond, :, :]
+            for eid in range(epoch.shape[1]):
+                r = np.sum(sub_epoch[eid, :])
+                if r > 0:
+                    start = np.nonzero(sub_epoch[eid, :])[0][0]
+                    epoch_info.append((cond, sid, start, start + r))
+    return epoch_info
+
+
+def _zscore_subjects_(processed_data, subject_count):
+    """z-score the epochs of each subject along the last axis, in place (subjects with one epoch are left as they are),
+    then ``nan_to_num`` (a constant voxel has sigma 0)."""
+    axis = processed_data.ndim - 1
+    cur_epoch = 0
+    for i in subject_count:
+        if i > 1:
+            processed_data[..., cur_epoch:cur_epoch + i] = \
+                zscore(processed_data[..., cur_epoch:cur_epoch + i], axis=axis, ddof=0)
+        cur_epoch += i
+    return np.nan_to_num(processed_data)
+
+
+def prepare_mvpa_data(images, conditions, mask):
+    """Drop-in for ``brainiak.fcma.preprocessing.prepare_mvpa_data`` (reference preprocessing.py:274-325): mask each
+    subject's image, average the activity within every epoch and z-score the epochs within subject.
+
+    Returns ``(processed_data, labels)``: float64 ``[num_voxels, num_epochs]`` and float64 ``[num_epochs]``."""
+    activity_data = [_mask_image(image, mask, np.float32) for image in images]
+    epoch_info = generate_epochs_info(conditions)
+    num_epochs = len(epoch_info)
+    (d1, _) = activity_data[0].shape
+    processed_data = np.empty([d1, num_epochs])
+    labels = np.empty(num_epochs)
+    subject_count = [0]
+    cur_sid = -1
+    for idx, epoch in enumerate(epoch_info):
+        labels[idx] = epoch[0]
+        if cur_sid != epoch[1]:
+            subject_count.append(0)
+            cur_sid = epoch[1]
+        subject_count[-1] += 1
+        processed_data[:, idx] = np.mean(activity_data[cur_sid][:, epoch[2]:epoch[3]], axis=1)
+    return _zscore_subjects_(processed_data, subject_count), labels
+
+
+def prepare_searchlight_mvpa_data(images, conditions, data_type=np.float32, random=RandomType.NORANDOM):
+    """Drop-in for ``brainiak.fcma.preprocessing.prepare_searchlight_mvpa_data`` (reference preprocessing.py:328-414):
+    the input of ``MVPAVoxelSelector``.  Averages the activity within every epoch and z-scores the epochs within
+    subject, keeping the 3-D brain; subjects are processed one at a time.  ``random`` shuffles each subject's voxels
+    (REPRODUCIBLE: seeded with the subject index).
+
+    Returns ``(processed_data, labels)``: ``data_type`` ``[X, Y, Z, num_epochs]`` and float64 ``[num_epochs]``."""
+    epoch_info = generate_epochs_info(conditions)
+    num_epochs = len(epoch_info)
+    processed_data = None
+    logger.info('there are %d subjects, and in total %d epochs', len(conditions), num_epochs)
+    labels = np.empty(num_epochs)
+    for idx, epoch in enumerate(epoch_info):
+        labels[idx] = epoch[0]
+    subject_count = np.zeros(len(conditions), dtype=np.int32)
+    for sid, f in enumerate(images):
+        data = (f.get_fdata() if hasattr(f, "get_fdata") else np.asarray(f)).astype(data_type)
+        if data.ndim != 4:
+            raise ValueError("image %d is not 4-D" % sid)
+        [d1, d2, d3, d4] = data.shape
+        if random != RandomType.NORANDOM:
+            data = data.reshape((d1 * d2 * d3, d4))
+            if random == RandomType.REPRODUCIBLE:
+                np.random.seed(sid)
+            np.random.shuffle(data)
+            data = data.reshape((d1, d2, d3, d4))
+        if processed_data is None:
+            processed_data = np.empty([d1, d2, d3, num_epochs], dtype=data_type)
+        for idx, epoch in enumerate(epoch_info):
+            if sid == epoch[1]:
+                subject_count[sid] += 1
+                processed_data[:, :, :, idx] = np.mean(data[:, :, :, epoch[2]:epoch[3]], axis=3)
+    return _zscore_subjects_(processed_data, subject_count), labels

@@ -215,6 +215,22 @@ int fcma_svm_cv_precomputed(const float *K_dev, long nv, int E, int nfolds, cons
 int fcma_svm_cv_solve(const float *K_dev, long nv, int E, int nproblems, const void *folds_host, double C, double tol,
                       int max_iter, int shrinking, int *correct_dev, unsigned long long *bits_dev, int *iters_dev,
                       void *stream);
+/* the same solver on fp64 kernels [nv][E][E]: Q_ab = (float)(y_a y_b K_fit_ab), QD_a = K_fit_aa and the decisions
+ * sum_k alpha_k y_k K_pred[t][k] - rho in double -- what libsvm computes for a non-precomputed kernel.  K_pred_dev may
+ * equal K_fit_dev (linear kernel). */
+int fcma_svm_cv_solve_f64(const double *K_fit_dev, const double *K_pred_dev, long nv, int E, int nproblems,
+                          const void *folds_host, double C, double tol, int max_iter, int shrinking, int *correct_dev,
+                          unsigned long long *bits_dev, int *iters_dev, void *stream);
+
+/* ---- searchlight kernel matrices (MVPAVoxelSelector, mvpa_voxelselector.py:34-49 per centre) --------------------------
+ * vol_dev: float32 [nx][ny][nz][E] (epochs contiguous per voxel); mask_dev: bytes [nx][ny][nz]; shape_dev: bytes
+ * [2r+1]^3; centres_host: M linear voxel indices, each at least sl_rad from every face; the features of a centre are
+ * the voxels of its cube where mask and shape hold, in C order.  K_fit_dev (and K_pred_dev for rbf): double [M][E][E].
+ * kind 0 linear: K_fit = G = sum_f x_a x_b.  kind 1 rbf with gamma_host[M]: K_fit = exp(-gamma ((G_aa + G_bb) - 2 G_ab)),
+ * K_pred = exp(-gamma sum_f (x_a - x_b)^2).  fp64 sums in cube order, no FMA contraction.  1 <= E <= 64. */
+int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E, const unsigned char *mask_dev,
+                             int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, int kind,
+                             const double *gamma_host, double *K_fit_dev, double *K_pred_dev, void *stream);
 
 /* ---- a12 / a15: plain NT GEMM  C[m][n] = sum_k A[m][k]*B[n][k]  (fp32 FFMA, row-major) ---------- */
 int fcma_gemm_nt(const float *A_dev, const float *B_dev, float *C_dev, long M, long N, long K,
