@@ -3399,6 +3399,71 @@ __device__ __forceinline__ void smo_pair_update(double &ai, double &aj, double y
     }
 }
 
+// libsvm's calculate_rho over positions [0, cnt) (lane l holds positions l and l + 32): the bounds' min / max in any
+// order, sum_free added sequentially in position order as libsvm's loop adds it; the same value on every lane
+__device__ __forceinline__ double svm_rho(const double (&y)[2], const double (&G)[2], const double (&alpha)[2], int cnt,
+                                          double C)
+{
+    const int lane = threadIdx.x & 31;
+    const double INF = __longlong_as_double(0x7ff0000000000000LL);
+    double ub = INF, lb = -INF, yG_free[2];
+    int nr_free = 0;
+#pragma unroll
+    for (int s = 0; s < 2; s++) {
+        yG_free[s] = 0.0;
+        if (lane + 32 * s >= cnt) continue;
+        const double yG = y[s] * G[s];
+        if (alpha[s] >= C) {
+            if (y[s] < 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
+        } else if (alpha[s] <= 0) {
+            if (y[s] > 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
+        } else {
+            ++nr_free;
+            yG_free[s] = yG;
+        }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        ub = fmin(ub, __shfl_xor_sync(0xffffffffu, ub, off));
+        lb = fmax(lb, __shfl_xor_sync(0xffffffffu, lb, off));
+        nr_free += __shfl_xor_sync(0xffffffffu, nr_free, off);
+    }
+    if (nr_free == 0) return (ub + lb) / 2;
+    double sum_free = 0.0;   // + 0.0 for a bounded position leaves the sum unchanged (it is never -0)
+    for (int k = 0; k < cnt; k++)
+        sum_free = __dadd_rn(sum_free, __shfl_sync(0xffffffffu, (k >> 5) ? yG_free[1] : yG_free[0], k & 31));
+    return sum_free / nr_free;
+}
+
+// The held-out decisions as libsvm's svm_predict_values forms them: dec = sum_k (alpha_k y_k) K(t, k) - rho with the
+// support vectors added sequentially in training order (class +1 first), each product and sum rounded on its own; dec > 0
+// -> the first class.  coef[k] = alpha_k y_k by training index k (per-warp shared memory).  Lane l predicts held-out
+// samples l and l + 32.  bits: bit t set when sample t falls on the first class's side; ok: correctly predicted samples.
+template <typename KT>
+__device__ __forceinline__ void svm_predict(const SvmFold &fd, const KT *__restrict__ Kp, int E, const double *coef,
+                                            double rho, int &ok, unsigned long long &bits)
+{
+    const int lane = threadIdx.x & 31;
+    bool pos[2], hit[2];
+#pragma unroll
+    for (int s = 0; s < 2; s++) {
+        const int t = lane + 32 * s;
+        pos[s] = hit[s] = false;
+        if (t >= fd.n_test) continue;
+        const KT *row = Kp + (size_t)fd.test_idx[t] * E;
+        double sum = 0.0;
+        for (int k = 0; k < fd.n_train; k++) {
+            const double c = coef[k];
+            if (c != 0.0) sum = __dadd_rn(sum, __dmul_rn(c, (double)row[fd.train_idx[k]]));
+        }
+        pos[s] = __dsub_rn(sum, rho) > 0;
+        hit[s] = pos[s] == (fd.test_pos[t] != 0);
+    }
+    bits = (unsigned long long)__ballot_sync(0xffffffffu, pos[0]) |
+           ((unsigned long long)__ballot_sync(0xffffffffu, pos[1]) << 32);
+    ok = __popc(__ballot_sync(0xffffffffu, hit[0])) + __popc(__ballot_sync(0xffffffffu, hit[1]));
+}
+
 // Kernel element type KT: float (the FCMA kernels) or double (searchlight kernels).  Either way Q is float and QD, the
 // gradient and the decisions are double, as libsvm keeps them; an fp64 kernel therefore reproduces what libsvm computes
 // for a non-precomputed kernel (QD and the decision values from the double kernel function).  The double form reads the
@@ -3515,7 +3580,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         }
         warp_argbest(obj_min, j, false);
         if (Gmax + Gmax2 < eps || j < 0) break;
-        if (max_iter > 0 && iter >= max_iter) break;
+        if (max_iter >= 0 && iter >= max_iter) break;
         ++iter;
 
         // ---- analytic update of (alpha_i, alpha_j) with libsvm's clipping
@@ -3539,46 +3604,18 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         }
     }
 
-    // ---- rho (calculate_rho)
-    double ub = INF, lb = -INF, sum_free = 0.0;
-    int nr_free = 0;
-#pragma unroll
-    for (int s = 0; s < 2; s++) {
-        if (!valid[s]) continue;
-        const double yG = y[s] * G[s];
-        if (alpha[s] >= C) {
-            if (y[s] < 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
-        } else if (alpha[s] <= 0) {
-            if (y[s] > 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
-        } else {
-            ++nr_free;
-            sum_free += yG;
-        }
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        ub = fmin(ub, __shfl_xor_sync(0xffffffffu, ub, off));
-        lb = fmax(lb, __shfl_xor_sync(0xffffffffu, lb, off));
-        sum_free += __shfl_xor_sync(0xffffffffu, sum_free, off);
-        nr_free += __shfl_xor_sync(0xffffffffu, nr_free, off);
-    }
-    const double rho = nr_free > 0 ? sum_free / nr_free : (ub + lb) / 2;
+    const double rho = svm_rho(y, G, alpha, n, C);
 
-    // ---- predict the held-out samples: dec = sum_k alpha_k y_k K(test, k) - rho;  dec > 0 -> class +
-    int ok = 0;
-    unsigned long long bits = 0ull;   // bit t: held-out sample t falls on the side of the first (smaller-label) class
-    for (int t = 0; t < fd.n_test; t++) {
-        const int it = fd.test_idx[t];
-        double part = 0.0;
+    // ---- predict the held-out samples; Q is no longer read, its space stages alpha_k y_k
+    double *coef = reinterpret_cast<double *>(Q);
+    __syncwarp();
 #pragma unroll
-        for (int s = 0; s < 2; s++)
-            if (valid[s] && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kp[(size_t)it * E + idx[s]];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
-        const bool pred_pos = (part - rho) > 0;
-        ok += (pred_pos == (fd.test_pos[t] != 0)) ? 1 : 0;
-        bits |= pred_pos ? (1ull << t) : 0ull;
-    }
+    for (int s = 0; s < 2; s++)
+        if (valid[s]) coef[lane + 32 * s] = alpha[s] * y[s];
+    __syncwarp();
+    int ok;
+    unsigned long long bits;
+    svm_predict(fd, Kp, E, coef, rho, ok, bits);
     if (lane == 0) {
         if (correct) correct[prob] = ok;
         if (iters) iters[prob] = iter;
@@ -3844,7 +3881,7 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
 
     int iter = 0;
     while (true) {
-        if (max_iter > 0 && iter >= max_iter) break;
+        if (max_iter >= 0 && iter >= max_iter) break;
         if (--counter == 0) {
             counter = n < 1000 ? n : 1000;
             do_shrinking();
@@ -3880,48 +3917,18 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
 #undef AT
 
     // ---- rho (calculate_rho over the active positions: all of them unless max_iter cut the loop)
-    double ub = INF, lb = -INF, sum_free = 0.0;
-    int nr_free = 0;
-#pragma unroll
-    for (int s = 0; s < 2; s++) {
-        const int k = lane + 32 * s;
-        if (k >= active) continue;
-        const double yG = y[s] * G[s];
-        if (alpha[s] >= C) {
-            if (y[s] < 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
-        } else if (alpha[s] <= 0) {
-            if (y[s] > 0) ub = fmin(ub, yG); else lb = fmax(lb, yG);
-        } else {
-            ++nr_free;
-            sum_free += yG;
-        }
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        ub = fmin(ub, __shfl_xor_sync(FULL, ub, off));
-        lb = fmax(lb, __shfl_xor_sync(FULL, lb, off));
-        sum_free += __shfl_xor_sync(FULL, sum_free, off);
-        nr_free += __shfl_xor_sync(FULL, nr_free, off);
-    }
-    const double rho = nr_free > 0 ? sum_free / nr_free : (ub + lb) / 2;
+    const double rho = svm_rho(y, G, alpha, active, C);
 
-    int ok = 0;
-    unsigned long long bits = 0ull;
-    int idx[2];
+    // ---- predict the held-out samples in training order: alpha_k y_k staged by unpermuted index pm in Q's space
+    double *coef = reinterpret_cast<double *>(Q);
+    __syncwarp();
 #pragma unroll
-    for (int s = 0; s < 2; s++) idx[s] = (lane + 32 * s) < n ? fd.train_idx[pm[s]] : 0;
-    for (int t = 0; t < fd.n_test; t++) {
-        const int it = fd.test_idx[t];
-        double part = 0.0;
-#pragma unroll
-        for (int s = 0; s < 2; s++)
-            if ((lane + 32 * s) < n && alpha[s] != 0.0) part += alpha[s] * y[s] * (double)Kp[(size_t)it * E + idx[s]];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(FULL, part, off);
-        const bool pred_pos = (part - rho) > 0;
-        ok += (pred_pos == (fd.test_pos[t] != 0)) ? 1 : 0;
-        bits |= pred_pos ? (1ull << t) : 0ull;
-    }
+    for (int s = 0; s < 2; s++)
+        if (lane + 32 * s < n) coef[pm[s]] = alpha[s] * y[s];
+    __syncwarp();
+    int ok;
+    unsigned long long bits;
+    svm_predict(fd, Kp, E, coef, rho, ok, bits);
     if (lane == 0) {
         if (correct) correct[prob] = ok;
         if (iters) iters[prob] = iter;

@@ -664,6 +664,11 @@ def _ovo_vote(bits, folds):
     return correct
 
 
+def _max_iter_arg(max_iter):
+    """SVC(max_iter) for the solver: -1 (any negative value, or None) runs without a limit, 0 runs no iteration."""
+    return -1 if max_iter is None or max_iter < 0 else int(max_iter)
+
+
 def svm_cv_precomputed(K, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, folds=None, return_iters=False,
                        shrinking=False):
     """Mean cross-validation accuracy of ``SVC(kernel='precomputed', C, tol, shrinking)`` for every kernel of
@@ -675,7 +680,7 @@ def svm_cv_precomputed(K, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, folds
     if folds is None:
         folds = make_svm_folds(labels, num_folds)
     nprob = folds.nproblems
-    cap = int(max_iter if max_iter and max_iter > 0 else 10000000)
+    cap = _max_iter_arg(max_iter)
     iters = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if return_iters else None
     two = len(folds.classes) == 2
     with torch.cuda.device(K.device):
@@ -708,7 +713,7 @@ def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, s
     if folds is None:
         folds = make_svm_folds(labels, num_folds)
     nprob = folds.nproblems
-    cap = int(max_iter if max_iter and max_iter > 0 else 10000000)
+    cap = _max_iter_arg(max_iter)
     two = len(folds.classes) == 2
     with torch.cuda.device(K_fit.device):
         iters = torch.empty((nv, nprob), dtype=torch.int32, device=K_fit.device) if return_iters else None

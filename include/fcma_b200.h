@@ -203,7 +203,11 @@ int fcma_shrink_kernels(float *K_dev, long nv, int E, int *digits_dev, void *str
  * (training samples of the smaller label first = class +1, as svm_group_classes orders them);
  * correct_dev[v*nfolds + f] = number of correctly predicted held-out samples; iters_dev optional.
  * E <= 64, at most 4096 fold problems, 2 <= n_train <= 64, n_test <= 64.  Replaces voxelselector.py:41-53 (_cross_validation_for_one_voxel)
- * as called by _do_cross_validation (voxelselector.py:423-465) for SVC(kernel='precomputed', shrinking=False). */
+ * as called by _do_cross_validation (voxelselector.py:423-465) for SVC(kernel='precomputed', shrinking=False).
+ * max_iter, here and in the two entry points below, is scikit-learn's SVC(max_iter): at most max_iter SMO iterations per
+ * problem, 0 runs none (every alpha stays 0, so rho = 0 and every decision is 0: the second class), and a negative value
+ * (-1) means no limit.  The held-out decisions sum alpha_k y_k K(t, k) sequentially in training order and rho sums the
+ * free variables in libsvm's order, so the decision values equal libsvm's bit for bit. */
 int fcma_svm_cv_precomputed(const float *K_dev, long nv, int E, int nfolds, const void *folds_host, double C,
                             double tol, int max_iter, int *correct_dev, int *iters_dev, void *stream);
 

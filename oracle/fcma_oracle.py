@@ -212,6 +212,14 @@ def svm_last_stats():
     return a.value, b.value
 
 
+def svm_last_detail():
+    """(reconstructions reading Q by rows, by columns, active set at the end) of the last svm_smo call: which loop orders
+    of libsvm's reconstruct_gradient ran, and whether a max_iter cut left variables shrunk."""
+    a, b, c = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
+    lib().oracle_svm_last_detail(ctypes.byref(a), ctypes.byref(b), ctypes.byref(c))
+    return a.value, b.value, c.value
+
+
 def svm_cv(K, labels, num_folds, C=1.0, tol=1e-3, shrinking=False):
     """cross_val_score(SVC(kernel='precomputed', C, tol, shrinking), K, labels, cv=StratifiedKFold(num_folds)) restated:
     scikit-learn's own splits, one-vs-one problems for more than two classes (pairs in libsvm's order, the smaller label is
@@ -235,8 +243,10 @@ def svm_cv(K, labels, num_folds, C=1.0, tol=1e-3, shrinking=False):
             idx = np.asarray(pos + neg)
             coef = alpha * np.r_[np.ones(len(pos)), -np.ones(len(neg))]
             for t, i in enumerate(te):
-                sv = alpha != 0
-                dec = float(np.sum(coef[sv] * K[i, idx[sv]].astype(np.float64))) - rho
+                dec = 0.0
+                for k in np.flatnonzero(alpha != 0):      # libsvm's svm_predict_values: training order, one by one
+                    dec = dec + float(coef[k]) * float(K[i, idx[k]])
+                dec -= rho
                 votes[t, a if dec > 0 else b] += 1
         pred = np.argmax(votes, axis=1)          # first maximum, as libsvm
         scores.append(float(np.mean(pred == code[te])))

@@ -22,6 +22,7 @@
 #define SMO_MAXN 64
 
 static __thread int g_min_active, g_reconstructs;   /* of the last solve on this thread: did the heuristic do anything? */
+static __thread int g_by_rows, g_by_cols, g_final_active;   /* reconstructions per loop order; active set at the end */
 
 typedef struct {
     int n, active, unshrink;
@@ -81,6 +82,7 @@ static void smo_reconstruct(smo_t *s)
     for (int k = s->active; k < n; k++) s->G[k] = s->Gbar[k] + (-1.0);
     for (int k = 0; k < s->active; k++) nr_free += !at_upper(s, k) && !at_lower(s, k);
     int by_rows = (long)nr_free * n > 2L * s->active * (n - s->active);
+    if (by_rows) ++g_by_rows; else ++g_by_cols;
     for (int jj = 0; jj < s->active; jj++) {
         if (at_upper(s, jj) || at_lower(s, jj)) continue;
         for (int k = s->active; k < n; k++)
@@ -170,6 +172,7 @@ int oracle_svm_smo(const float *K, int E, const int *train_idx, int n, int n_pos
     float *Q = (float *)malloc(sizeof(float) * n * n);
     g_min_active = n;
     g_reconstructs = 0;
+    g_by_rows = g_by_cols = 0;
     s.n = s.active = n;
     s.unshrink = 0;
     s.C = C;
@@ -188,7 +191,7 @@ int oracle_svm_smo(const float *K, int E, const int *train_idx, int n, int n_pos
     int iter = 0, counter = (n < 1000 ? n : 1000) + 1;
     for (;;) {
         int i, j;
-        if (max_iter > 0 && iter >= max_iter) break;
+        if (max_iter >= 0 && iter >= max_iter) break;   /* scikit-learn: -1 = no limit, 0 = no iteration */
         if (--counter == 0) {
             counter = n < 1000 ? n : 1000;
             if (shrinking) smo_shrink(&s);
@@ -223,6 +226,7 @@ int oracle_svm_smo(const float *K, int E, const int *train_idx, int n, int n_pos
         else { ++nr_free; sum_free += yG; }
     }
     *rho_out = nr_free > 0 ? sum_free / nr_free : (ub + lb) / 2;
+    g_final_active = s.active;
     for (int k = 0; k < n; k++) alpha_out[s.pm[k]] = s.alpha[k];
     free(Q);
     return iter;
@@ -243,4 +247,13 @@ void oracle_svm_last_stats(int *min_active, int *reconstructs)
 {
     *min_active = g_min_active;
     *reconstructs = g_reconstructs;
+}
+
+/* of the last oracle_svm_smo call on this thread: gradient reconstructions that read Q by rows / by columns, and the
+ * active set when the loop ended (below n when max_iter cut it while variables were shrunk) */
+void oracle_svm_last_detail(int *by_rows, int *by_cols, int *final_active)
+{
+    *by_rows = g_by_rows;
+    *by_cols = g_by_cols;
+    *final_active = g_final_active;
 }
