@@ -487,7 +487,6 @@ constexpr int GEMM_MAX_STAGES = 8;
 
 struct GemmParams {
     int E, Kp, bk, mma_k, kbs;
-    int segs, seg_r[3], seg_c[3], planes;
     long V2, nb, row_start;
     int tiles_j, tiles_i;          // 256 x 256 tiles
     long total_tiles;
@@ -598,6 +597,25 @@ __device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t da, uint
     else wgmma_m64n256_tf32(d, da, db, scale_d);
 }
 
+// One k-block of a tile as one straight-line wgmma group: NK k-steps of every product, in prec_info's order (small cross
+// terms first, hi * hi last; one product with one plane).  The fence and the commit are part of the batch: with them
+// after the caller's switch on NK, ptxas closes a group at the end of each case and the commit adds an empty one.
+template <int FMT, int PLANES, int NK>
+__device__ __forceinline__ void corr_batch(float (&d)[128], uint32_t cols, uint32_t rows, uint32_t scale_first)
+{
+    constexpr int SEGS = PLANES == 2 ? 3 : 1;
+    wgmma_fence();
+#pragma unroll
+    for (int sgm = 0; sgm < SEGS; sgm++) {
+        const int pc = PLANES == 2 && sgm == 1, pr = PLANES == 2 && sgm == 0;   // seg_c {0, 1, 0}, seg_r {1, 0, 0}
+        const uint64_t da = make_wgmma_desc_sw128(cols + pc * 16384);
+        const uint64_t db = make_wgmma_desc_sw128(rows + pr * 32768);
+#pragma unroll
+        for (int k = 0; k < NK; k++) wgmma_m64n256<FMT>(d, da + 2 * k, db + 2 * k, sgm == 0 && k == 0 ? scale_first : 1u);
+    }
+    wgmma_commit();
+}
+
 // tile t of this launch -> (epoch, column tile, row tile); false: a mirrored tile of the symmetric diagonal block
 __device__ __forceinline__ bool gemm_tile_coords(const GemmParams &p, long tile, int &e, int &tj, int &ti)
 {
@@ -610,7 +628,7 @@ __device__ __forceinline__ bool gemm_tile_coords(const GemmParams &p, long tile,
     return !(p.sym_diag && tj < ti);
 }
 
-template <int FMT, bool HALF_OUT>
+template <int FMT, int PLANES, bool HALF_OUT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     k_corr_wgmma(const __grid_constant__ CUtensorMap tm_cols, const __grid_constant__ CUtensorMap tm_rows,
                  const GemmParams p)
@@ -653,9 +671,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_expect_tx(&full_bar[stage], p.stage_bytes);
                     uint8_t *base = smem + (size_t)stage * p.stage_bytes;
-                    for (int pl = 0; pl < p.planes; pl++) {
+                    for (int pl = 0; pl < PLANES; pl++) {
                         tma_load_3d(&tm_cols, &full_bar[stage], base + pl * 16384, k0, col0, pl * p.E + e);
-                        tma_load_3d(&tm_rows, &full_bar[stage], base + p.planes * 16384 + pl * 32768, k0, row0,
+                        tma_load_3d(&tm_rows, &full_bar[stage], base + PLANES * 16384 + pl * 32768, k0, row0,
                                     pl * p.E + e);
                     }
                     if (++stage == p.stages) {
@@ -678,26 +696,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         for (long tile = pair; tile < p.total_tiles; tile += npairs) {
             int e, tj, ti;
             if (!gemm_tile_coords(p, tile, e, tj, ti)) continue;
-            uint32_t accumulate = 0;
             for (int kb = 0; kb < p.kbs; kb++) {
                 mbar_wait(&full_bar[stage], phase);
                 const uint32_t base = tiles_addr + (uint32_t)stage * p.stage_bytes;
-                const uint32_t rbase = base + p.planes * 16384;
+                const uint32_t cols = base + cw * 8192, rows = base + PLANES * 16384;
                 const int rem_k = p.Kp - kb * p.bk;
-                const int nk = (rem_k < p.bk ? rem_k : p.bk) / p.mma_k;
-                wgmma_fence();
-                for (int sgm = 0; sgm < p.segs; sgm++) {
-                    const uint64_t da = make_wgmma_desc_sw128(base + p.seg_c[sgm] * 16384 + cw * 8192);
-                    const uint64_t db = make_wgmma_desc_sw128(rbase + p.seg_r[sgm] * 32768);
-#pragma unroll
-                    for (int k = 0; k < 4; k++) {   // bk / mma_k == 4 for every operand format: 32 bytes per k-step
-                        if (k < nk) {
-                            wgmma_m64n256<FMT>(acc, da + 2 * k, db + 2 * k, accumulate);
-                            accumulate = 1;
-                        }
-                    }
+                const uint32_t scale_first = kb > 0;
+                switch ((rem_k < p.bk ? rem_k : p.bk) / p.mma_k) {   // bk / mma_k == 4 for every format: 32 B per k-step
+                case 1: corr_batch<FMT, PLANES, 1>(acc, cols, rows, scale_first); break;
+                case 2: corr_batch<FMT, PLANES, 2>(acc, cols, rows, scale_first); break;
+                case 3: corr_batch<FMT, PLANES, 3>(acc, cols, rows, scale_first); break;
+                default: corr_batch<FMT, PLANES, 4>(acc, cols, rows, scale_first); break;
                 }
-                wgmma_commit();
                 wgmma_wait_all();
                 mbar_arrive(&empty_bar[stage]);
                 if (++stage == p.stages) {
@@ -821,8 +831,6 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     GemmParams q;
     memset(&q, 0, sizeof(q));
     q.E = E, q.Kp = Kp, q.bk = pi.bk, q.mma_k = pi.mma_k, q.kbs = (int)cdiv(Kp, pi.bk);
-    q.segs = pi.segs, q.planes = pi.planes;
-    for (int sgm = 0; sgm < 3; sgm++) q.seg_r[sgm] = pi.seg_r[sgm], q.seg_c[sgm] = pi.seg_c[sgm];
     q.V2 = V2, q.nb = nb, q.row_start = start;
     q.col_start = sym ? start : 0;
     q.tiles_j = (int)cdiv(V2 - q.col_start, 256), q.tiles_i = (int)cdiv(nb, 256);
@@ -873,8 +881,20 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     auto gemm = [&](auto kernel) {
         rc = launch_kernel(kernel, (unsigned)(2 * pairs), GEMM_THREADS, smem, st, "k_corr_wgmma", tm_cols, tm_rows, q);
     };
-    if (!with_int<0, 1, 2>(pi.fmt, [&](auto FMT) { half_out ? gemm(k_corr_wgmma<FMT, true>) : gemm(k_corr_wgmma<FMT, false>); }))
-        return fail(FCMA_EINVAL, "internal: no k_corr_wgmma instantiation for operand type %d", pi.fmt);
+    // the kernel compiles the product order in (corr_batch): one product with one plane, prec_info's three with two
+    const bool order_ok = pi.planes == 1 ? pi.segs == 1
+                                         : pi.segs == 3 && pi.seg_r[0] == 1 && pi.seg_r[1] == 0 && pi.seg_r[2] == 0 &&
+                                               pi.seg_c[0] == 0 && pi.seg_c[1] == 1 && pi.seg_c[2] == 0;
+    auto go = [&](auto FMT, auto PLANES) {
+        half_out ? gemm(k_corr_wgmma<FMT, PLANES, true>) : gemm(k_corr_wgmma<FMT, PLANES, false>);
+    };
+    if (!order_ok) return fail(FCMA_EINVAL, "internal: k_corr_wgmma has no product order for precision %d", precision);
+    if (pi.fmt == 0 && pi.planes == 2) go(IntC<0>{}, IntC<2>{});        // fp16x3
+    else if (pi.fmt == 1 && pi.planes == 1) go(IntC<1>{}, IntC<1>{});   // bf16
+    else if (pi.fmt == 1 && pi.planes == 2) go(IntC<1>{}, IntC<2>{});   // bf16x3
+    else if (pi.fmt == 2 && pi.planes == 1) go(IntC<2>{}, IntC<1>{});   // tf32
+    else if (pi.fmt == 2 && pi.planes == 2) go(IntC<2>{}, IntC<2>{});   // tf32x3
+    else return fail(FCMA_EINVAL, "internal: no k_corr_wgmma instantiation for operand type %d, %d planes", pi.fmt, pi.planes);
     if (rc) return rc;
 
     if (rows_op == cols_op && V == V2 && fixup) {
