@@ -1050,6 +1050,30 @@ __global__ void __launch_bounds__(256) k_row_normalize(float *X, long R, long D,
 // ============================================================================================
 // a6 standalone: exact restatement of fcma_extension.cc:52-84 (sequential fp32, no FMA contraction)
 // ============================================================================================
+// Fisher-z and z-score, in place, of subject s's epochs [s*eps, (s+1)*eps) of one column: mat[b * ld] is epoch b.  The one
+// copy of this arithmetic: k_within_subject_norm and k_norm_gram_f64 (the per-voxel fp64 kernels of VoxelSelector's
+// feature path) both call it, so their z values are bit-identical.
+__device__ __forceinline__ void within_subject_column(float *mat, long ld, long s, int eps)
+{
+    float mean = 0.0f, sq = 0.0f;
+    for (long b = s * eps; b < (s + 1) * eps; b++) {
+        float r = mat[(size_t)b * ld];
+        float num = __fadd_rn(1.0f, r);
+        float den = __fsub_rn(1.0f, r);
+        num = (num <= 0.0f) ? 1e-4f : num;
+        den = (den <= 0.0f) ? 1e-4f : den;
+        float z = __fmul_rn(0.5f, logf(__fdiv_rn(num, den)));
+        mat[(size_t)b * ld] = z;
+        mean = __fadd_rn(mean, z);
+        sq = __fadd_rn(sq, __fmul_rn(z, z));
+    }
+    mean = __fdiv_rn(mean, (float)eps);
+    float var = __fsub_rn(__fdiv_rn(sq, (float)eps), __fmul_rn(mean, mean));
+    float inv = (var <= 0.0f) ? 0.0f : __fdiv_rn(1.0f, __fsqrt_rn(var));
+    for (long b = s * eps; b < (s + 1) * eps; b++)
+        mat[(size_t)b * ld] = __fmul_rn(__fsub_rn(mat[(size_t)b * ld], mean), inv);
+}
+
 __global__ void __launch_bounds__(256) k_within_subject_norm(float *data, long n0, int E, long n2, int eps)
 {
     const long nSubjs = E / eps;
@@ -1059,24 +1083,7 @@ __global__ void __launch_bounds__(256) k_within_subject_norm(float *data, long n
         const long v = idx / n2;
         const long s = v % nSubjs;
         const long i = v / nSubjs;
-        float *mat = data + (size_t)i * E * n2 + j;
-        float mean = 0.0f, sq = 0.0f;
-        for (long b = s * eps; b < (s + 1) * eps; b++) {
-            float r = mat[(size_t)b * n2];
-            float num = __fadd_rn(1.0f, r);
-            float den = __fsub_rn(1.0f, r);
-            num = (num <= 0.0f) ? 1e-4f : num;
-            den = (den <= 0.0f) ? 1e-4f : den;
-            float z = __fmul_rn(0.5f, logf(__fdiv_rn(num, den)));
-            mat[(size_t)b * n2] = z;
-            mean = __fadd_rn(mean, z);
-            sq = __fadd_rn(sq, __fmul_rn(z, z));
-        }
-        mean = __fdiv_rn(mean, (float)eps);
-        float var = __fsub_rn(__fdiv_rn(sq, (float)eps), __fmul_rn(mean, mean));
-        float inv = (var <= 0.0f) ? 0.0f : __fdiv_rn(1.0f, __fsqrt_rn(var));
-        for (long b = s * eps; b < (s + 1) * eps; b++)
-            mat[(size_t)b * n2] = __fmul_rn(__fsub_rn(mat[(size_t)b * n2], mean), inv);
+        within_subject_column(data + (size_t)i * E * n2 + j, n2, s, eps);
     }
 }
 
@@ -2885,12 +2892,22 @@ static bool half_block(int precision, int flags)
     return half;
 }
 
-// shared body of the two fused pipelines
+// Second stage of fcma_voxel_feature_kernels: the per-voxel fp64 kernel matrices of the normalised correlation vectors
+// (k_norm_gram_f64) instead of the fp32 SYRK.  kind 0 linear, 1 rbf; outputs [nb][E][E].
+struct FeatureStage {
+    int kind;
+    double gamma;
+    double *K_fit, *K_pred;
+};
+static int launch_norm_gram_f64(const float *C, long nb, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
+                                int eps, int kind, double gamma, double *K_fit, double *K_pred, cudaStream_t st);
+
+// shared body of the fused pipelines; with `feat` the GEMM writes raw r and the feature stage replaces normalise+SYRK
 static int run_pipeline(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2, long start,
                         long nb, int eps, int flags, float *work, size_t work_bytes, float *K, int sum_over_rows,
-                        cudaStream_t st)
+                        cudaStream_t st, const FeatureStage *feat = nullptr)
 {
-    if (!rows_op || !cols_op || !work || !K) return fail(FCMA_EINVAL, "pipeline: null pointer");
+    if (!rows_op || !cols_op || !work || !(K || feat)) return fail(FCMA_EINVAL, "pipeline: null pointer");
     if (nb <= 0 || start < 0 || start + nb > V) return fail(FCMA_EINVAL, "pipeline: rows [%ld, %ld) outside [0, %ld)", start, start + nb, V);
     if (eps < 0) return fail(FCMA_EINVAL, "pipeline: negative epochs_per_subj");
     if (((uintptr_t)work & 15)) return fail(FCMA_EINVAL, "pipeline: work buffer must be 16-byte aligned");
@@ -2903,16 +2920,16 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
     const bool normalise = sum_over_rows ? eps > 1 : eps >= 1;
     const bool fused = normalise ? fused_supported(E, eps) : fused_supported(E, 0);
     const int S_eps = normalise ? (E / eps) * eps : 0;
-    const bool fisher_in_gemm = normalise && fused && !(flags & FCMA_FLAG_FISHER_IN_PASS2);
+    const bool fisher_in_gemm = !feat && normalise && fused && !(flags & FCMA_FLAG_FISHER_IN_PASS2);
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
-    if (mask_self && !(normalise && fused))
+    if (mask_self && (feat || !(normalise && fused)))
         return fail(FCMA_EINVAL, "FCMA_FLAG_MASK_SELF needs the fused normalise+kernel path (E <= 64, power-of-two eps)");
     // Tiled intermediate [n/256][T256][E][256][256]: every 256x256 pair tile of the GEMM is one contiguous 256 KB
     // run and the E tiles of one (row block, column block) are adjacent, so the fused normalise+SYRK kernel reads
     // row i as E runs of 1 KB, 256 KB apart, inside one 8 MB region.  Needs whole 256-row blocks of workspace.
     // FCMA_FLAG_STRIDED_BLOCK keeps the strided [i][e][j] block.
     const long t256 = cdiv(V2, 256);
-    const bool tiled = !(flags & FCMA_FLAG_STRIDED_BLOCK) && fused && V2 < (1L << 31) && rows_per_pass >= 256;
+    const bool tiled = !(flags & FCMA_FLAG_STRIDED_BLOCK) && (fused || feat) && V2 < (1L << 31) && rows_per_pass >= 256;
     // an fp16 block needs the tiled layout and holds Fisher-z values (applied in the GEMM epilogue)
     const bool half16 = half_block(precision, flags) && tiled && normalise && fisher_in_gemm;
     for (long done = 0; done < nb; done += rows_per_pass) {
@@ -2931,7 +2948,13 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
         if (rc) return rc;
         float *Kdst = sum_over_rows ? K : K + (size_t)done * E * E;
         const float beta = sum_over_rows ? 1.0f : 0.0f;
-        if (tiled) {
+        if (feat) {
+            const size_t off = (size_t)done * E * E;
+            rc = tiled ? launch_norm_gram_f64(work, n, E, V2, 256, 65536, (long)E * 65536, t256, eps, feat->kind, feat->gamma,
+                                              feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st)
+                       : launch_norm_gram_f64(work, n, E, V2, (long)E * ld, ld, 256, t256, eps, feat->kind, feat->gamma,
+                                              feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st);
+        } else if (tiled) {
             rc = launch_norm_syrk(work, n, E, V2, 256, 65536, normalise ? eps : 0, (normalise && fisher_in_gemm) ? 1 : 0,
                                   mask_self ? start + done : -1, beta, Kdst, sum_over_rows, st, (long)E * 65536,
                                   half16 ? 1 : 0);
@@ -4052,6 +4075,15 @@ static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int
 #define SL_CHUNK 32
 #define SL_PAIRS 9   // ceil(64 * 65 / 2 / SL_THREADS)
 
+// libsvm's rbf kernel values from fp64 sums, each operation rounded separately: the x_square form its training uses
+// (from the Gram entries G_aa, G_bb, G_ab; exactly 1 on the diagonal) and the difference form of its decisions (from
+// d = sum_f (x_a - x_b)^2).  Shared by k_searchlight_kernels and k_norm_gram_f64.
+__device__ __forceinline__ double rbf_fit(double gamma, double gaa, double gbb, double gab)
+{
+    return exp(__dmul_rn(-gamma, __dsub_rn(__dadd_rn(gaa, gbb), __dmul_rn(2.0, gab))));
+}
+__device__ __forceinline__ double rbf_pred(double gamma, double d) { return exp(__dmul_rn(-gamma, d)); }
+
 template <int KIND>
 __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float *__restrict__ vol, int ny, int nz, int E,
                                                                     const unsigned char *__restrict__ mask, int r,
@@ -4134,7 +4166,7 @@ __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float 
     for (int s = 0; s < SL_PAIRS; s++) {
         if (pa[s] < 0) continue;
         double v = g[s];
-        if (KIND == 1) v = exp(__dmul_rn(-gm, __dsub_rn(__dadd_rn(diag[pa[s]], diag[pb[s]]), __dmul_rn(2.0, g[s]))));
+        if (KIND == 1) v = rbf_fit(gm, diag[pa[s]], diag[pb[s]], g[s]);
         tile[pa[s] * E + pb[s]] = v;
         tile[pb[s] * E + pa[s]] = v;
     }
@@ -4145,7 +4177,7 @@ __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float 
 #pragma unroll
         for (int s = 0; s < SL_PAIRS; s++) {
             if (pa[s] < 0) continue;
-            const double v = exp(__dmul_rn(-gm, d[s]));
+            const double v = rbf_pred(gm, d[s]);
             tile[pa[s] * E + pb[s]] = v;
             tile[pb[s] * E + pa[s]] = v;
         }
@@ -4193,6 +4225,209 @@ extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, 
                              K_pred_dev);
     return launch_kernel(k_searchlight_kernels<1>, (unsigned)M, SL_THREADS, smem, st, "k_searchlight_kernels", vol_dev,
                          (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev, K_pred_dev);
+}
+
+// ============================================================================================
+// Per-voxel fp64 kernel matrices of the normalised correlation vectors (VoxelSelector with SVC(kernel='linear' | 'rbf')):
+// for voxel row i of a raw correlation block, z = within_subject_column(r) (bit-identical to k_within_subject_norm), then
+//   G_ab = sum_j z_aj z_bj          on the fp64 tensor cores (mma.sync m8n8k4 f64; fp32 products are exact in fp64)
+//   D_ab = sum_j (z_aj - z_bj)^2    rbf only, on the FP64 pipe (difference in fp64, then one fma)
+// and the epilogue: linear K_fit = G; rbf K_fit = rbf_fit(G), K_pred = rbf_pred(D).  These are the kernel values libsvm
+// computes for SVC(kernel=...) on the float32 features z, up to the order of the sums (DESIGN.md §3.8).
+//
+// One CTA per row (grid-stride).  The row's E x V2 block streams through shared memory in chunks of NG_CH columns: loaded
+// one chunk ahead into registers, normalised in place as fp32 [E][NG_RSP], widened to fp64 transposed [NG_CH][EP + 4]
+// (EP = E rounded up to 16, zero rows past E; the pad makes both the MMA fragments and the D rows conflict-free).
+// G: the NB8 = EP/8 row blocks of 8 give NB8(NB8+1)/2 upper 8x8 tiles; warp w takes the tile rows p and NB8-1-p
+// (p = w % (NB8/2): NB8+1 tiles, the same for every warp) over every WK-th k-step (WK = 16/NB8 k-groups), and the k-groups'
+// partial tiles are added in k-group order at the end of the row.  D: thread q < 136 owns the entries (ty + 16u, tx + 16v),
+// ty <= tx, of a 16 x 16 grid, each summed sequentially over j.  No atomics: two runs are bit-identical.
+#define NG_THREADS 256
+#define NG_CH 64        // columns per chunk; divides the 256-column tiles of the tiled block
+#define NG_RSP 72       // fp32 row pitch of the chunk (conflict-free in both the normalisation and the widening)
+
+__device__ __forceinline__ void dmma_m8n8k4(double (&d)[2], double a, double b)
+{
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};\n"
+                 : "+d"(d[0]), "+d"(d[1])
+                 : "d"(a), "d"(b));
+}
+
+// E > 32: 36 G tiles + 16 D sums per thread do not fit the 128 registers of two CTAs per SM without spills
+template <int EP, int KIND>
+__global__ void __launch_bounds__(NG_THREADS, EP == 64 ? 1 : 2)
+    k_norm_gram_f64(const float *__restrict__ C, long nb, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
+                    int eps, double gamma, double *__restrict__ K_fit, double *__restrict__ K_pred)
+{
+    constexpr int NB8 = EP / 8, NP = NB8 / 2, WK = 8 / NP, RPT = EP / 16, LDT = EP + 4, NPF = EP / 16;
+    extern __shared__ double s_ng[];
+    double *zt = s_ng;                                             // [NG_CH][LDT] z (fp64), then the [EP][EP] result tile
+    float *rs = reinterpret_cast<float *>(zt + NG_CH * LDT);       // [E][NG_RSP] the chunk of r, normalised in place
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int p = warp % NP, kq = warp / NP;
+    const long nsubj = E / eps;
+    int ty = 0, tx = 0;
+    const bool dq = KIND == 1 && tid < 136;
+    if (dq) {
+        int q = tid;
+        while (q >= 16 - ty) q -= 16 - ty++;
+        tx = ty + q;
+    }
+    for (long i = blockIdx.x; i < nb; i += gridDim.x) {
+        const float *Ci = C + (chunk_step != 256 ? (i / 256) * t256 * chunk_step + (i % 256) * stride_i : i * stride_i);
+        float4 pf[NPF];
+        auto prefetch = [&](long j0) {
+            const float *src = Ci + (j0 / 256) * chunk_step + j0 % 256;
+#pragma unroll
+            for (int k = 0; k < NPF; k++) {
+                const int idx = tid + k * NG_THREADS, e = idx / (NG_CH / 4), c4 = idx % (NG_CH / 4);
+                pf[k] = (e < E && j0 + 4 * c4 < n2) ? __ldg(reinterpret_cast<const float4 *>(src + e * ld + 4 * c4))
+                                                    : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+        };
+        double acc[NB8 + 1][2];
+        double dacc[RPT][RPT];
+#pragma unroll
+        for (int u = 0; u <= NB8; u++) acc[u][0] = acc[u][1] = 0.0;
+#pragma unroll
+        for (int a = 0; a < RPT; a++)
+#pragma unroll
+            for (int b = 0; b < RPT; b++) dacc[a][b] = 0.0;
+        prefetch(0);
+        for (long j0 = 0; j0 < n2; j0 += NG_CH) {
+            __syncthreads();   // the previous chunk (and the previous row's result tile) is consumed
+#pragma unroll
+            for (int k = 0; k < NPF; k++) {
+                const int idx = tid + k * NG_THREADS, e = idx / (NG_CH / 4), c4 = idx % (NG_CH / 4);
+                float4 v = pf[k];
+                // columns past n2 (inside the last float4, or pad of the block) are zero: they add nothing to G or D
+                const long j = j0 + 4 * c4;
+                if (j + 1 >= n2) v.y = 0.f;
+                if (j + 2 >= n2) v.z = 0.f;
+                if (j + 3 >= n2) v.w = 0.f;
+                if (e < E) *reinterpret_cast<float4 *>(rs + e * NG_RSP + 4 * c4) = v;
+            }
+            if (j0 + NG_CH < n2) prefetch(j0 + NG_CH);
+            __syncthreads();
+            // epochs past the last whole subject keep their raw r, as in k_within_subject_norm
+            for (int idx = tid; idx < nsubj * NG_CH; idx += NG_THREADS)
+                within_subject_column(rs + idx % NG_CH, NG_RSP, idx / NG_CH, eps);
+            __syncthreads();
+            for (int idx = tid; idx < EP * NG_CH; idx += NG_THREADS) {
+                const int grp = idx >> 5, l = idx & 31;
+                const int e = (grp % (EP / 4)) * 4 + (l & 3), c = (grp / (EP / 4)) * 8 + (l >> 2);
+                zt[c * LDT + e] = e < E ? (double)rs[e * NG_RSP + c] : 0.0;
+            }
+            __syncthreads();
+            for (int ks = kq; ks < NG_CH / 4; ks += WK) {
+                const double *zk = zt + (ks * 4 + t) * LDT + g;
+                const double fa = zk[p * 8], fb = zk[(NB8 - 1 - p) * 8];
+#pragma unroll
+                for (int u = 0; u <= NB8; u++) {
+                    // tiles (p, p..NB8-1), then (NB8-1-p, NB8-1-p..NB8-1)
+                    const bool first = u < NB8 - p;
+                    dmma_m8n8k4(acc[u], first ? fa : fb, zk[(first ? p + u : u - 1) * 8]);
+                }
+            }
+            if (dq) {
+                for (int c = 0; c < NG_CH; c++) {
+                    const double *zc = zt + c * LDT;
+                    double za[RPT], zb[RPT];
+#pragma unroll
+                    for (int u = 0; u < RPT; u++) za[u] = zc[ty + 16 * u], zb[u] = zc[tx + 16 * u];
+#pragma unroll
+                    for (int a = 0; a < RPT; a++)
+#pragma unroll
+                        for (int b = 0; b < RPT; b++) {
+                            const double df = __dsub_rn(za[a], zb[b]);
+                            dacc[a][b] = __fma_rn(df, df, dacc[a][b]);
+                        }
+                }
+            }
+        }
+        // epilogue: G into the [EP][EP] tile (upper 8x8 tiles only), k-groups added in order
+        double *tile = zt;
+        for (int r = 0; r < WK; r++) {
+            __syncthreads();
+            if (kq == r) {
+#pragma unroll
+                for (int u = 0; u <= NB8; u++) {
+                    const bool first = u < NB8 - p;
+                    const int rb = first ? p : NB8 - 1 - p, cb = first ? p + u : u - 1;
+                    double *dst = tile + (rb * 8 + g) * EP + cb * 8 + 2 * t;
+                    dst[0] = r == 0 ? acc[u][0] : __dadd_rn(dst[0], acc[u][0]);
+                    dst[1] = r == 0 ? acc[u][1] : __dadd_rn(dst[1], acc[u][1]);
+                }
+            }
+        }
+        __syncthreads();
+        const size_t base = (size_t)i * E * E;
+        for (int idx = tid; idx < E * E; idx += NG_THREADS) {
+            const int a = idx / E, b = idx - a * E;
+            double v = tile[min(a, b) * EP + max(a, b)];
+            if (KIND == 1) v = rbf_fit(gamma, tile[a * EP + a], tile[b * EP + b], v);
+            K_fit[base + idx] = v;
+        }
+        if (KIND == 1) {
+            __syncthreads();
+            if (dq) {
+#pragma unroll
+                for (int a = 0; a < RPT; a++)
+#pragma unroll
+                    for (int b = 0; b < RPT; b++) {
+                        tile[(ty + 16 * a) * EP + tx + 16 * b] = dacc[a][b];
+                        tile[(tx + 16 * b) * EP + ty + 16 * a] = dacc[a][b];
+                    }
+            }
+            __syncthreads();
+            for (int idx = tid; idx < E * E; idx += NG_THREADS) {
+                const int a = idx / E, b = idx - a * E;
+                K_pred[base + idx] = rbf_pred(gamma, tile[a * EP + b]);
+            }
+        }
+    }
+}
+
+// (stride_i, ld, chunk_step, t256) address the raw correlation block as launch_norm_syrk's do (tiled: chunk_step = E*65536)
+static int launch_norm_gram_f64(const float *C, long nb, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
+                                int eps, int kind, double gamma, double *K_fit, double *K_pred, cudaStream_t st)
+{
+    if (E < 1 || E > 64 || eps < 1) return fail(FCMA_EINVAL, "internal: k_norm_gram_f64 needs 1 <= E <= 64, eps >= 1");
+    if (((uintptr_t)C & 15) || (ld & 3) || (stride_i & 3)) return fail(FCMA_EINVAL, "internal: k_norm_gram_f64 needs 16-byte rows");
+    const long grid = nb < 16L * g_sm_count ? nb : 16L * g_sm_count;
+    bool ok = false;
+    int rc = FCMA_OK;
+    auto go = [&](auto EP, auto KIND) {
+        constexpr size_t smem = (size_t)NG_CH * (EP + 4) * sizeof(double) + (size_t)EP * NG_RSP * sizeof(float);
+        rc = launch_kernel(k_norm_gram_f64<EP, KIND>, (unsigned)grid, NG_THREADS, smem, st, "k_norm_gram_f64", C, nb, E, n2,
+                           stride_i, ld, chunk_step, t256, eps, gamma, K_fit, K_pred);
+        ok = true;
+    };
+    auto per_kind = [&](auto EP) {
+        if (kind == 0) go(EP, IntC<0>{});
+        else go(EP, IntC<1>{});
+    };
+    if (E <= 16) per_kind(IntC<16>{});
+    else if (E <= 32) per_kind(IntC<32>{});
+    else per_kind(IntC<64>{});
+    return ok ? rc : fail(FCMA_EINVAL, "internal: no k_norm_gram_f64 instantiation for E=%d", E);
+}
+
+extern "C" int fcma_voxel_feature_kernels(const void *rows_op, const void *cols_op, int precision, int E, int T, long V,
+                                          long V2, long start, long nb, int eps, int kind, double gamma, float *work_dev,
+                                          size_t work_bytes, double *K_fit_dev, double *K_pred_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (eps <= 0) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: epochs_per_subj must be positive");
+    if (E < 1 || E > 64) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: E = %d outside 1..64", E);
+    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: kind must be 0 (linear) or 1 (rbf)");
+    if (!K_fit_dev || (kind == 1 && !K_pred_dev)) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: null output");
+    if (kind == 1 && !(gamma >= 0.0 && gamma <= 1.7976931348623157e308))
+        return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: gamma must be finite and non-negative");
+    FeatureStage fs{kind, gamma, K_fit_dev, K_pred_dev};
+    return run_pipeline(rows_op, cols_op, precision, E, T, V, V2, start, nb, eps, 0, work_dev, work_bytes, nullptr, 0,
+                        (cudaStream_t)stream, &fs);
 }
 
 // ---------------------------------------------------------------- host-buffer entry points

@@ -309,6 +309,37 @@ def voxel_kernels(rows, cols, start, nb, eps, flags=0, work=None, out=None):
     return out
 
 
+def feature_kernels_f64(rows, cols, start, nb, eps, kind="linear", gamma=None, work=None):
+    """a4 -> a6 -> fp64 kernel matrices of the normalised correlation vectors for voxel rows [start, start+nb)
+    (fcma_voxel_feature_kernels): z[i] is the ``[E, V2]`` block ``within_subject_norm_`` gives on the raw correlations,
+    bit for bit.  ``kind='linear'``: returns ``(G, G)``, ``G_ab = sum_j z_aj z_bj``; ``kind='rbf'`` with a number
+    ``gamma``: ``(K_fit, K_pred)``, the x_square form libsvm trains with and the difference form of its decisions.  Both
+    float64 CUDA ``[nb, E, E]``, ready for ``svm_cv_f64``; the result is that of ``SVC(kernel=kind)`` on the features."""
+    lib = _lib.load()
+    _check_pair(rows, cols)
+    E, V2 = rows.E, cols.V
+    if kind not in ("linear", "rbf"):
+        raise ValueError("kind must be 'linear' or 'rbf', not %r" % (kind,))
+    kcode = 0 if kind == "linear" else 1
+    g = 0.0
+    if kcode == 1:
+        if gamma is None:
+            raise ValueError("kind='rbf' needs gamma")
+        g = float(gamma)
+        if not (np.isfinite(g) and g >= 0):
+            raise ValueError("gamma must be finite and non-negative")
+    if work is None:
+        work = Workspace(E, V2, Workspace.rows_for(E, V2, nb, rows.device), rows.device)
+    K_fit = torch.empty((nb, E, E), dtype=torch.float64, device=rows.device)
+    K_pred = K_fit if kcode == 0 else torch.empty_like(K_fit)
+    with torch.cuda.device(rows.device):
+        _lib.check(lib.fcma_voxel_feature_kernels(_ptr(rows.buf), _ptr(cols.buf), _prec_code(rows.precision), E, rows.T,
+                                                  rows.V, V2, start, nb, int(eps), kcode, g, _ptr(work.buf),
+                                                  work.buf.numel(), _ptr(K_fit), _ptr(K_pred) if kcode else None,
+                                                  _stream_ptr()))
+    return K_fit, K_pred
+
+
 def sym_row_partition(num_voxels, world_size, align=256, pack_frac=0.01):
     """Shards of [0, V) for the symmetric pipeline.  Shard r contracts its rows with the columns at or to the right of
     its first row, so the work of rows [a, b) is the trapezoid area (1 - a/V)^2 - (1 - b/V)^2 of the upper triangle, plus
@@ -587,6 +618,35 @@ def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True):
     except ValueError:
         return False
     return True
+
+
+def svc_feature_kind(clf, labels, num_folds, E):
+    """``'linear'`` / ``'rbf'`` if ``cross_val_score(clf, X, labels, cv=StratifiedKFold(num_folds))`` on float32
+    features ``X`` (E samples) can be computed as ``svm_cv_f64`` on the fp64 kernel matrices of ``X``, else None:
+    ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')`` with ``gamma='auto'`` or a number >= 0, without class weights,
+    probability or tie breaking, E <= 64, at most 64 folds that ``make_svm_folds`` accepts.  ``gamma='scale'`` depends on
+    the variance of the training features and stays with scikit-learn."""
+    import numbers
+    import sklearn.svm
+    if not isinstance(clf, sklearn.svm.SVC):
+        return None
+    if clf.kernel == 'linear':
+        kind = 'linear'
+    elif clf.kernel == 'rbf' and (clf.gamma == 'auto' or (isinstance(clf.gamma, numbers.Real)
+                                                          and not isinstance(clf.gamma, bool) and clf.gamma >= 0)):
+        kind = 'rbf'
+    else:
+        return None
+    # scikit-learn >= 1.9 uses the string 'deprecated' as the default of `probability`
+    if clf.class_weight is not None or getattr(clf, 'probability', False) is True or getattr(clf, 'break_ties', False):
+        return None
+    if E > 64 or num_folds > 64:
+        return None
+    try:
+        make_svm_folds(labels, num_folds)
+    except ValueError:
+        return None
+    return kind
 
 
 class SvmFolds:

@@ -13,10 +13,8 @@ classifier (``gamma='scale'``, poly, sigmoid, other estimators), float64 data, m
 cannot express or ``gpu_cv=False`` run the reference's per-centre ``cross_val_score`` on the host.
 """
 import logging
-import numbers
 
 import numpy as np
-import sklearn.svm
 from sklearn import model_selection
 
 from .. import _lib
@@ -82,29 +80,11 @@ class MVPAVoxelSelector:
     # ------------------------------------------------------------------ routing
     def _gpu_kind(self, clf):
         """'linear' / 'rbf' if ``clf`` and the data can be scored on the GPU, else None."""
-        if not self.gpu_cv or not isinstance(clf, sklearn.svm.SVC):
+        if not self.gpu_cv:
             return None
-        if clf.kernel == 'linear':
-            kind = 'linear'
-        elif clf.kernel == 'rbf' and (clf.gamma == 'auto' or (isinstance(clf.gamma, numbers.Real)
-                                                              and not isinstance(clf.gamma, bool)
-                                                              and clf.gamma >= 0)):
-            kind = 'rbf'
-        else:
-            return None
-        # scikit-learn >= 1.9 uses the string 'deprecated' as the default of `probability`
-        if clf.class_weight is not None or getattr(clf, 'probability', False) is True \
-                or getattr(clf, 'break_ties', False):
-            return None
-        if np.asarray(self.data).dtype != np.float32:
+        kind = engine.svc_feature_kind(clf, self.labels, self.num_folds, self.data.shape[3])
+        if kind is not None and np.asarray(self.data).dtype != np.float32:
             logger.info('MVPAVoxelSelector: data is %s, not float32: scoring on the host', np.asarray(self.data).dtype)
-            return None
-        E = self.data.shape[3]
-        if E > 64 or self.num_folds > 64:
-            return None
-        try:
-            engine.make_svm_folds(self.labels, self.num_folds)
-        except ValueError:
             return None
         return kind
 

@@ -7,8 +7,9 @@ accuracy, descending), same private stage methods.  The three native stages of
 
     corr GEMM (TMA + wgmma)  ->  Fisher-z + within-subject z-score  ->  per-voxel E x E kernel
 
-The cross validation itself (voxelselector.py:41-53, scikit-learn) stays on the host, exactly as in
-the reference.  Distribution: instead of the MPI master/worker farm (voxelselector.py:176-282) every
+The cross validation runs on the GPU for ``SVC(kernel='precomputed')`` on the kernel matrices and for
+``SVC(kernel='linear' | 'rbf')`` on the normalised correlation vectors (see ``gpu_cv``); any other classifier is
+cross-validated on the host by scikit-learn, exactly as in the reference (voxelselector.py:41-53).  Distribution: instead of the MPI master/worker farm (voxelselector.py:176-282) every
 rank of ``torch.distributed`` owns a contiguous slice of voxel rows (work per row is uniform); the
 per-voxel scores are gathered on ``master_rank``.  Without ``torch.distributed`` it runs on one GPU.
 """
@@ -91,11 +92,15 @@ class VoxelSelector:
         (engine.voxel_kernels_sym; half the tensor work, same kernels up to fp32 summation order).  Over
         several GPUs the shards' partial kernel arrays are summed with one NCCL reduce-scatter (every rank keeps the
         rows it cross-validates).
-    gpu_cv: run the voxelwise cross validation of an ``SVC(kernel='precomputed')`` on the GPU (batched restatement of
-        libsvm's SMO, with or without its shrinking heuristic as ``clf.shrinking`` says, with the same iterations and
-        decisions as scikit-learn; more than two conditions one-vs-one with libsvm's vote, see
-        engine.svm_cv_precomputed); ``False`` or any other classifier -> scikit-learn on the host, exactly as the
-        reference (voxelselector.py:41-53)
+    gpu_cv: run the voxelwise cross validation on the GPU (batched restatement of libsvm's SMO, with or without its
+        shrinking heuristic as ``clf.shrinking`` says, with the same iterations and decisions as scikit-learn; more than
+        two conditions one-vs-one with libsvm's vote, see engine.svm_cv_precomputed) for
+        ``SVC(kernel='precomputed')`` on the kernel matrices, and for ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')``
+        with ``gamma='auto'`` or a number on the normalised correlation vectors themselves: their fp64 kernel matrices
+        are built on the GPU (engine.feature_kernels_f64, without the decimal shrink, as scikit-learn sees the features)
+        and cross-validated by engine.svm_cv_f64 (at most 64 epochs and folds, no class weights, probability or tie
+        breaking, and ``mask_self=False``, see engine.svc_feature_kind).  ``False`` or any other classifier ->
+        scikit-learn on the host, exactly as the reference (voxelselector.py:41-53)
     """
 
     def __init__(self, labels, epochs_per_subj, num_folds, raw_data, raw_data2=None,
@@ -337,21 +342,51 @@ class VoxelSelector:
             results += self._cv_block(K[s - k0:s - k0 + nb], s, nb, clf, on_gpu, folds)
         return results
 
+    def _plain_block(self, n):
+        """Rows per pass of the plain (row-block) pipeline, with its scratch allocated for them."""
+        rows_op, _ = self._operands()
+        E = rows_op.E
+        block = self.block_rows or engine.Workspace.rows_for(E, self.num_voxels2, n, rows_op.device)
+        block = max(1, min(block, n))
+        if self._work is None or self._work.rows < block or isinstance(self._work, engine.SymWorkspace):
+            self._work = None
+            self._work = engine.Workspace(E, self.num_voxels2, block, rows_op.device)
+        return block
+
+    def _feature_kind(self, clf):
+        """'linear' / 'rbf' when ``clf`` on the normalised correlation vectors is cross-validated on the GPU (fp64 kernel
+        matrices + the fp64 solver), else None.  mask_self is not applied to the features by the host path, so that
+        combination stays there."""
+        if not self.gpu_cv or self.mask_self:
+            return None
+        return engine.svc_feature_kind(clf, self.labels, self.num_folds, len(self.raw_data))
+
     def _score_rows(self, start, n, clf):
-        """GPU stages for rows [start, start+n) in HBM-sized blocks, then host CV."""
+        """GPU stages for rows [start, start+n) in HBM-sized blocks, then the cross validation (GPU or host)."""
         import torch
         rows_op, cols_op = self._operands()
         E = rows_op.E
         results = []
         if _is_precomputed_svc(clf) and self._symmetric_ok():
             return self._score_rows_symmetric(start, n, clf)
-        if _is_precomputed_svc(clf):
+        kind = None if _is_precomputed_svc(clf) else self._feature_kind(clf)
+        if kind is not None:
+            # SVC(kernel='linear' | 'rbf') on the features: the fp64 kernels of the features give libsvm's iterations and
+            # decisions (DESIGN.md §3.8); gamma='auto' is scikit-learn's 1 / n_features
+            gamma = None if kind == 'linear' else (1.0 / self.num_voxels2 if clf.gamma == 'auto' else float(clf.gamma))
+            folds = engine.make_svm_folds(self.labels, self.num_folds)
+            block = self._plain_block(n)
+            for s in range(start, start + n, block):
+                nb = min(block, start + n - s)
+                K_fit, K_pred = engine.feature_kernels_f64(rows_op, cols_op, s, nb, self.epochs_per_subj, kind, gamma,
+                                                           work=self._work)
+                acc = engine.svm_cv_f64(K_fit, K_pred, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
+                                        max_iter=clf.max_iter, shrinking=bool(clf.shrinking), folds=folds)
+                del K_fit, K_pred
+                results += [(int(s + k), acc[k]) for k in range(nb)]
+        elif _is_precomputed_svc(clf):
             fused = engine.fused_supported(E, self.epochs_per_subj)
-            block = self.block_rows or engine.Workspace.rows_for(E, self.num_voxels2, n, rows_op.device)
-            block = max(1, min(block, n))
-            if self._work is None or self._work.rows < block or isinstance(self._work, engine.SymWorkspace):
-                self._work = None
-                self._work = engine.Workspace(E, self.num_voxels2, block, rows_op.device)
+            block = self._plain_block(n)
             on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E)
             folds = engine.make_svm_folds(self.labels, self.num_folds) if on_gpu else None
             for s in range(start, start + n, block):

@@ -236,6 +236,19 @@ int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, in
                              int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, int kind,
                              const double *gamma_host, double *K_fit_dev, double *K_pred_dev, void *stream);
 
+/* ---- per-voxel fp64 kernels of the normalised correlation vectors (VoxelSelector with SVC(kernel='linear' | 'rbf')) ----
+ * The plain pipeline of fcma_voxel_kernels (one or two masks, same operands, work buffer and passes) with a different
+ * second stage.  For voxel rows [start, start+nb): z[i] = the raw correlations r[i] ([E][V2]) normalised exactly as
+ * fcma_within_subject_norm does (any eps >= 1; epochs past the last whole subject keep their raw r), then, in fp64,
+ * G_ab = sum_j z_aj z_bj and, for rbf, D_ab = sum_j (z_aj - z_bj)^2, in a fixed order (two runs are bit-identical).
+ *   kind 0 linear: K_fit = G (K_pred_dev may be null).
+ *   kind 1 rbf:    K_fit = exp(-gamma ((G_aa + G_bb) - 2 G_ab)), K_fit_aa = 1; K_pred = exp(-gamma D).  gamma >= 0, finite.
+ * These are the kernel values libsvm computes for SVC(kernel=...) on the float32 features z[i], so fcma_svm_cv_solve_f64
+ * on them cross-validates that classifier.  Outputs double [nb][E][E]; 1 <= E <= 64. */
+int fcma_voxel_feature_kernels(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2,
+                               long start, long nb, int eps, int kind, double gamma, float *work_dev, size_t work_bytes,
+                               double *K_fit_dev, double *K_pred_dev, void *stream);
+
 /* ---- a12 / a15: plain NT GEMM  C[m][n] = sum_k A[m][k]*B[n][k]  (fp32 FFMA, row-major) ---------- */
 int fcma_gemm_nt(const float *A_dev, const float *B_dev, float *C_dev, long M, long N, long K,
                  long lda, long ldb, long ldc, void *stream);
