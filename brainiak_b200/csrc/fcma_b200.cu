@@ -3353,14 +3353,27 @@ __global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E
 // select_working_set :946-1043 (WSS2, ">=" / "<=" tie-breaking = last index), calculate_rho
 // :1126-1162, float Q values, double gradient, eps = tol, TAU = 1e-12; classes grouped with the
 // smaller label first = +1 (svm_group_classes :2246-2326); prediction dec > 0 -> first class
-// :2842-2905), without the shrinking heuristic (identical result for shrinking=False, equal within
-// tol otherwise).  Lane l owns training samples l and l+32 (n_train <= 64).
+// :2842-2905), with or without the shrinking heuristic (a template switch of k_svm_cv).  Lane l owns
+// training samples l and l+32 (n_train <= 64).
 struct SvmFold {
     int n_train, n_pos, n_test, pad;
     int train_idx[64];        // class (+1) samples first, original order inside a class
     int test_idx[64];
     unsigned char test_pos[64];
 };
+
+// A warp's staging area in the shrinking solver: do_shrinking moves the items' state between positions through it
+struct SvmStage {
+    double d[4][64];          // G, G_bar, alpha, QD by position
+    int i[2][64];             // pm, y > 0
+    unsigned char map[64];    // map[new position] = old position
+};
+// Dynamic shared memory of a k_svm_cv block (4 warps): the warps' Q [64][64] floats, then with shrinking their stages
+constexpr int SVM_Q_FLOATS = 4 * 64 * 64;
+constexpr size_t svm_smem_bytes(bool shrink)
+{
+    return SVM_Q_FLOATS * sizeof(float) + (shrink ? 4 * sizeof(SvmStage) : 0);
+}
 
 __device__ __forceinline__ void warp_argbest(double &val, int &idx, bool want_max)
 {
@@ -3374,6 +3387,13 @@ __device__ __forceinline__ void warp_argbest(double &val, int &idx, bool want_ma
             idx = oi;
         }
     }
+}
+
+// The value at position pos of an array held lane-slot-wise (lane l holds positions l and l + 32), on every lane
+template <typename T>
+__device__ __forceinline__ T warp_at(const T (&a)[2], int pos)
+{
+    return __shfl_sync(0xffffffffu, (pos >> 5) ? a[1] : a[0], pos & 31);
 }
 
 // libsvm's analytic two-variable step with its clipping order (Solver::Solve, "update alpha[i] and alpha[j]")
@@ -3473,8 +3493,7 @@ __device__ __forceinline__ double svm_rho(const double (&y)[2], const double (&G
     }
     if (nr_free == 0) return (ub + lb) / 2;
     double sum_free = 0.0;   // + 0.0 for a bounded position leaves the sum unchanged (it is never -0)
-    for (int k = 0; k < cnt; k++)
-        sum_free = __dadd_rn(sum_free, __shfl_sync(0xffffffffu, (k >> 5) ? yG_free[1] : yG_free[0], k & 31));
+    for (int k = 0; k < cnt; k++) sum_free = __dadd_rn(sum_free, warp_at(yG_free, k));
     return sum_free / nr_free;
 }
 
@@ -3512,13 +3531,20 @@ __device__ __forceinline__ void svm_predict(const SvmFold &fd, const KT *__restr
 // for a non-precomputed kernel (QD and the decision values from the double kernel function).  The double form reads the
 // decisions' kernel values from Kpred (the rbf difference form of k_function); the float form ignores Kpred.  Q is
 // formed as y_a y_b (float)K, which equals (float)(y_a y_b K) because y_a y_b = +-1 and rounding commutes with the sign.
-template <typename KT>
+//
+// SHRINK adds libsvm's shrinking heuristic (scikit-learn's default shrinking=True): Solver::do_shrinking, be_shrunk,
+// reconstruct_gradient, swap_index and the counter / unshrink logic of Solver::Solve restated for one warp.  Lanes own
+// POSITIONS lane and lane+32 of libsvm's permuted arrays; an item's state (y, alpha, G, G_bar, QD and its index `pm` in
+// the unpermuted sub-problem = active_set[]) travels between positions through the warp's SvmStage when do_shrinking
+// swaps; Q stays in the unpermuted order and is addressed through pm.  Working-set selection, the G update and rho run
+// over [0, active); G_bar over all n.  Without SHRINK, active = n and every item stays at its own position.
+template <typename KT, bool SHRINK>
 __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long nv, int E, int nfolds,
                                                const SvmFold *__restrict__ folds, double C, double eps, int max_iter,
                                                int *__restrict__ correct, int *__restrict__ iters,
                                                unsigned long long *__restrict__ dec_bits, const KT *__restrict__ Kpred)
 {
-    extern __shared__ float s_q[];   // [4 warps][nmax][nmax]
+    extern __shared__ float s_q[];   // svm_smem_bytes(SHRINK): [4 warps][64][64] Q, then with SHRINK [4 warps] SvmStage
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long prob = (long)blockIdx.x * 4 + warp;
     if (prob >= nv * nfolds) return;
@@ -3529,182 +3555,32 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
     const KT *Kv = K + (size_t)v * E * E;
     const KT *Kp = sizeof(KT) == 4 ? Kv : Kpred + (size_t)v * E * E;
     float *Q = s_q + (size_t)warp * 64 * 64;
-    const double INF = __longlong_as_double(0x7ff0000000000000LL);
-    const double TAU = 1e-12;
-
-    // sub-problem in libsvm's order; Q_ab = (float)(y_a y_b K_ab)
-    int idx[2];
-    double y[2], alpha[2], G[2], QD[2];
-    bool valid[2];
-#pragma unroll
-    for (int s = 0; s < 2; s++) {
-        const int k = lane + 32 * s;
-        valid[s] = k < n;
-        idx[s] = valid[s] ? fd.train_idx[k] : 0;
-        y[s] = k < fd.n_pos ? 1.0 : -1.0;
-        alpha[s] = 0.0;
-        G[s] = -1.0;   // p = -1
-    }
-    for (int a = 0; a < n; a++) {
-        const int ia = fd.train_idx[a];
-        const float ya = a < fd.n_pos ? 1.f : -1.f;
-#pragma unroll
-        for (int s = 0; s < 2; s++) {
-            const int k = lane + 32 * s;
-            if (valid[s]) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + idx[s]];
-        }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int s = 0; s < 2; s++) QD[s] = valid[s] ? (double)Kv[(size_t)idx[s] * E + idx[s]] : 0.0;
-
-    int iter = 0;
-    while (true) {
-        // ---- working set selection (second order)
-        double Gmax = -INF;
-        int i = -1;
-#pragma unroll
-        for (int s = 0; s < 2; s++) {
-            if (!valid[s]) continue;
-            double cand = -INF;
-            if (y[s] > 0) {
-                if (!(alpha[s] >= C)) cand = -G[s];
-            } else {
-                if (!(alpha[s] <= 0)) cand = G[s];
-            }
-            if (cand >= Gmax && cand > -INF) {
-                Gmax = cand;
-                i = lane + 32 * s;
-            }
-        }
-        warp_argbest(Gmax, i, true);
-        if (i < 0) break;
-        const double yi = i < fd.n_pos ? 1.0 : -1.0;
-        const double QDi = __shfl_sync(0xffffffffu, (i >> 5) ? QD[1] : QD[0], i & 31);
-        double Gmax2 = -INF, obj_min = INF;
-        int j = -1;
-#pragma unroll
-        for (int s = 0; s < 2; s++) {
-            if (!valid[s]) continue;
-            const int k = lane + 32 * s;
-            const double Qik = (double)Q[i * 64 + k];
-            if (y[s] > 0) {
-                if (!(alpha[s] <= 0)) {
-                    const double gd = Gmax + G[s];
-                    if (G[s] >= Gmax2) Gmax2 = G[s];
-                    if (gd > 0) {
-                        const double quad = QDi + QD[s] - 2.0 * yi * Qik;
-                        const double obj = quad > 0 ? -(gd * gd) / quad : -(gd * gd) / TAU;
-                        if (obj <= obj_min) {
-                            j = k;
-                            obj_min = obj;
-                        }
-                    }
-                }
-            } else {
-                if (!(alpha[s] >= C)) {
-                    const double gd = Gmax - G[s];
-                    if (-G[s] >= Gmax2) Gmax2 = -G[s];
-                    if (gd > 0) {
-                        const double quad = QDi + QD[s] + 2.0 * yi * Qik;
-                        const double obj = quad > 0 ? -(gd * gd) / quad : -(gd * gd) / TAU;
-                        if (obj <= obj_min) {
-                            j = k;
-                            obj_min = obj;
-                        }
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            double o = __shfl_xor_sync(0xffffffffu, Gmax2, off);
-            Gmax2 = o > Gmax2 ? o : Gmax2;
-        }
-        warp_argbest(obj_min, j, false);
-        if (Gmax + Gmax2 < eps || j < 0) break;
-        if (max_iter >= 0 && iter >= max_iter) break;
-        ++iter;
-
-        // ---- analytic update of (alpha_i, alpha_j) with libsvm's clipping
-        const double yj = j < fd.n_pos ? 1.0 : -1.0;
-        const double QDj = __shfl_sync(0xffffffffu, (j >> 5) ? QD[1] : QD[0], j & 31);
-        const double Gi = __shfl_sync(0xffffffffu, (i >> 5) ? G[1] : G[0], i & 31);
-        const double Gj = __shfl_sync(0xffffffffu, (j >> 5) ? G[1] : G[0], j & 31);
-        double ai = __shfl_sync(0xffffffffu, (i >> 5) ? alpha[1] : alpha[0], i & 31);
-        double aj = __shfl_sync(0xffffffffu, (j >> 5) ? alpha[1] : alpha[0], j & 31);
-        const double old_ai = ai, old_aj = aj;
-        smo_pair_update(ai, aj, yi, yj, QDi, QDj, (double)Q[i * 64 + j], Gi, Gj, C);
-        const double dai = ai - old_ai, daj = aj - old_aj;
-#pragma unroll
-        for (int s = 0; s < 2; s++) {
-            if (!valid[s]) continue;
-            const int k = lane + 32 * s;
-            // G[k] += Q_i[k]*dai + Q_j[k]*daj, no FMA contraction (as the reference compiles it)
-            G[s] = __dadd_rn(G[s], __dadd_rn(__dmul_rn((double)Q[i * 64 + k], dai), __dmul_rn((double)Q[j * 64 + k], daj)));
-            if (k == i) alpha[s] = ai;
-            if (k == j) alpha[s] = aj;
-        }
-    }
-
-    const double rho = svm_rho(y, G, alpha, n, C);
-
-    // ---- predict the held-out samples; Q is no longer read, its space stages alpha_k y_k
-    double *coef = reinterpret_cast<double *>(Q);
-    __syncwarp();
-#pragma unroll
-    for (int s = 0; s < 2; s++)
-        if (valid[s]) coef[lane + 32 * s] = alpha[s] * y[s];
-    __syncwarp();
-    int ok;
-    unsigned long long bits;
-    svm_predict(fd, Kp, E, coef, rho, ok, bits);
-    if (lane == 0) {
-        if (correct) correct[prob] = ok;
-        if (iters) iters[prob] = iter;
-        if (dec_bits) dec_bits[prob] = bits;
-    }
-}
-
-// ---- the same solver WITH libsvm's shrinking heuristic (scikit-learn's default shrinking=True): Solver::do_shrinking,
-// be_shrunk, reconstruct_gradient, swap_index and the counter / unshrink logic of Solver::Solve restated for one warp.
-// Lanes own POSITIONS lane and lane+32 of libsvm's permuted arrays; an item's state (y, alpha, G, G_bar, QD and its
-// index `pm` in the unpermuted sub-problem = active_set[]) travels between positions through a shared staging area when
-// do_shrinking swaps; Q stays in the unpermuted order and is addressed through pm.  Working-set selection, the G update
-// and rho run over [0, active); G_bar over all n.
-template <typename KT>
-__global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K, long nv, int E, int nfolds,
-                                                      const SvmFold *__restrict__ folds, double C, double eps,
-                                                      int max_iter, int *__restrict__ correct, int *__restrict__ iters,
-                                                      unsigned long long *__restrict__ dec_bits,
-                                                      const KT *__restrict__ Kpred)
-{
-    extern __shared__ float s_q[];   // [4 warps][64][64] Q, then per warp: 4 x 64 doubles, 2 x 64 ints, 64 bytes
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long prob = (long)blockIdx.x * 4 + warp;
-    if (prob >= nv * nfolds) return;
-    const long v = prob / nfolds;
-    const int f = (int)(prob - v * nfolds);
-    const SvmFold &fd = folds[f];
-    const int n = fd.n_train;
-    const KT *Kv = K + (size_t)v * E * E;
-    const KT *Kp = sizeof(KT) == 4 ? Kv : Kpred + (size_t)v * E * E;
-    float *Q = s_q + (size_t)warp * 64 * 64;
-    double *stg_d = reinterpret_cast<double *>(s_q + 4 * 64 * 64) + warp * 4 * 64;
-    int *stg_i = reinterpret_cast<int *>(reinterpret_cast<double *>(s_q + 4 * 64 * 64) + 4 * 4 * 64) + warp * 2 * 64;
-    unsigned char *map =
-        reinterpret_cast<unsigned char *>(reinterpret_cast<int *>(reinterpret_cast<double *>(s_q + 4 * 64 * 64) + 4 * 4 * 64) + 4 * 2 * 64) +
-        warp * 64;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
     const double TAU = 1e-12;
     const unsigned FULL = 0xffffffffu;
 
+    // the item at a position: its index in the unpermuted sub-problem (Q's row / column) and its y, on every lane; and
+    // the index of this lane's slot s.  Without shrinking that is the position itself and y follows from it.
     int pm[2];
-    double y[2], alpha[2], G[2], Gb[2], QD[2];
+    double y[2];
+    auto index_at = [&](int pos) {
+        if constexpr (SHRINK) return warp_at(pm, pos); else return pos;
+    };
+    auto own_index = [&](int s) {
+        if constexpr (SHRINK) return pm[s]; else return lane + 32 * s;
+    };
+    auto y_at = [&](int pos) {
+        if constexpr (SHRINK) return warp_at(y, pos); else return pos < fd.n_pos ? 1.0 : -1.0;
+    };
+
+    // sub-problem in libsvm's order; Q_ab = (float)(y_a y_b K_ab)
+    int idx[2];
+    double alpha[2], G[2], Gb[2], QD[2];
 #pragma unroll
     for (int s = 0; s < 2; s++) {
         const int k = lane + 32 * s;
         pm[s] = k < n ? k : 0;
+        idx[s] = k < n ? fd.train_idx[k] : 0;
         y[s] = k < fd.n_pos ? 1.0 : -1.0;
         alpha[s] = 0.0;
         G[s] = -1.0;   // p = -1
@@ -3716,23 +3592,18 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
-            if (k < n) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + fd.train_idx[k]];
+            if (k < n) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + idx[s]];
         }
     }
     __syncwarp();
 #pragma unroll
-    for (int s = 0; s < 2; s++) {
-        const int k = lane + 32 * s;
-        const int ik = k < n ? fd.train_idx[k] : 0;
-        QD[s] = k < n ? (double)Kv[(size_t)ik * E + ik] : 0.0;
-    }
+    for (int s = 0; s < 2; s++) QD[s] = lane + 32 * s < n ? (double)Kv[(size_t)idx[s] * E + idx[s]] : 0.0;
 
     int active = n;
     bool unshrink = false;
     int counter = (n < 1000 ? n : 1000) + 1;
-#define AT(arr, pos) __shfl_sync(FULL, ((pos) >> 5) ? arr[1] : arr[0], (pos) & 31)
 
-    // Solver::select_working_set over [0, active); true = already optimal (libsvm returns 1)
+    // Solver::select_working_set (second order) over [0, active); true = already optimal (libsvm returns 1)
     auto select = [&](int &i, int &j) -> bool {
         double Gmax = -INF;
         i = -1;
@@ -3754,14 +3625,14 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
         warp_argbest(Gmax, i, true);
         j = -1;
         if (i < 0) return true;
-        const double yi = AT(y, i), QDi = AT(QD, i);
-        const int pmi = AT(pm, i);
+        const double yi = y_at(i), QDi = warp_at(QD, i);
+        const float *Qi = Q + index_at(i) * 64;
         double Gmax2 = -INF, obj_min = INF;
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
             if (k >= active) continue;
-            const double Qik = (double)Q[pmi * 64 + pm[s]];
+            const double Qik = (double)Qi[own_index(s)];
             if (y[s] > 0) {
                 if (!(alpha[s] <= 0)) {
                     const double gd = Gmax + G[s];
@@ -3814,8 +3685,8 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
         for (int off = 16; off > 0; off >>= 1) nr_free += __shfl_xor_sync(FULL, nr_free, off);
         const bool by_rows = (long)nr_free * n > 2L * active * (n - active);
         for (int jj = 0; jj < active; jj++) {
-            const double a_j = AT(alpha, jj);
-            const int pm_j = AT(pm, jj);
+            const double a_j = warp_at(alpha, jj);
+            const int pm_j = warp_at(pm, jj);
             if (a_j >= C || a_j <= 0) continue;
 #pragma unroll
             for (int s = 0; s < 2; s++) {
@@ -3869,8 +3740,9 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
         unsigned long long F = (unsigned long long)__ballot_sync(FULL, fl[0]) |
                                ((unsigned long long)__ballot_sync(FULL, fl[1]) << 32);
         if (F == 0ull) return;
-        map[lane] = (unsigned char)lane;
-        map[lane + 32] = (unsigned char)(lane + 32);
+        SvmStage &stg = reinterpret_cast<SvmStage *>(s_q + SVM_Q_FLOATS)[warp];
+        stg.map[lane] = (unsigned char)lane;
+        stg.map[lane + 32] = (unsigned char)(lane + 32);
         __syncwarp();
         int act = active, swaps = 0;
         if (lane == 0) {
@@ -3881,9 +3753,9 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
                     act--;
                     while (act > i) {
                         if (!((F >> act) & 1ull)) {
-                            const unsigned char t = map[i];
-                            map[i] = map[act];
-                            map[act] = t;
+                            const unsigned char t = stg.map[i];
+                            stg.map[i] = stg.map[act];
+                            stg.map[act] = t;
                             F ^= (1ull << i) | (1ull << act);
                             ++swaps;
                             break;
@@ -3899,25 +3771,25 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
-            stg_d[k] = G[s];
-            stg_d[64 + k] = Gb[s];
-            stg_d[128 + k] = alpha[s];
-            stg_d[192 + k] = QD[s];
-            stg_i[k] = pm[s];
-            stg_i[64 + k] = y[s] > 0 ? 1 : 0;
+            stg.d[0][k] = G[s];
+            stg.d[1][k] = Gb[s];
+            stg.d[2][k] = alpha[s];
+            stg.d[3][k] = QD[s];
+            stg.i[0][k] = pm[s];
+            stg.i[1][k] = y[s] > 0 ? 1 : 0;
         }
         __syncwarp();
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
             if (k >= n) continue;
-            const int src = map[k];
-            G[s] = stg_d[src];
-            Gb[s] = stg_d[64 + src];
-            alpha[s] = stg_d[128 + src];
-            QD[s] = stg_d[192 + src];
-            pm[s] = stg_i[src];
-            y[s] = stg_i[64 + src] ? 1.0 : -1.0;
+            const int src = stg.map[k];
+            G[s] = stg.d[0][src];
+            Gb[s] = stg.d[1][src];
+            alpha[s] = stg.d[2][src];
+            QD[s] = stg.d[3][src];
+            pm[s] = stg.i[0][src];
+            y[s] = stg.i[1][src] ? 1.0 : -1.0;
         }
         __syncwarp();
     };
@@ -3925,49 +3797,59 @@ __global__ void __launch_bounds__(128) k_svm_cv_shrink(const KT *__restrict__ K,
     int iter = 0;
     while (true) {
         if (max_iter >= 0 && iter >= max_iter) break;
-        if (--counter == 0) {
-            counter = n < 1000 ? n : 1000;
-            do_shrinking();
-        }
         int i, j;
-        if (select(i, j)) {
-            reconstruct();
-            active = n;
-            if (select(i, j)) break;
-            counter = 1;   // do shrinking next iteration
+        if constexpr (SHRINK) {
+            if (--counter == 0) {
+                counter = n < 1000 ? n : 1000;
+                do_shrinking();
+            }
+            if (select(i, j)) {
+                reconstruct();
+                active = n;
+                if (select(i, j)) break;
+                counter = 1;   // do shrinking next iteration
+            }
+        } else if (select(i, j)) {
+            break;
         }
         ++iter;
-        const double yi = AT(y, i), yj = AT(y, j), QDi = AT(QD, i), QDj = AT(QD, j);
-        const double Gi = AT(G, i), Gj = AT(G, j);
-        const int pmi = AT(pm, i), pmj = AT(pm, j);
-        double ai = AT(alpha, i), aj = AT(alpha, j);
+
+        // ---- analytic update of (alpha_i, alpha_j) with libsvm's clipping, then G (and G_bar) of every position
+        const double yi = y_at(i), yj = y_at(j), QDi = warp_at(QD, i), QDj = warp_at(QD, j);
+        const double Gi = warp_at(G, i), Gj = warp_at(G, j);
+        const int pmi = index_at(i), pmj = index_at(j);
+        const float *Qi = Q + pmi * 64, *Qj = Q + pmj * 64;
+        double ai = warp_at(alpha, i), aj = warp_at(alpha, j);
         const double old_ai = ai, old_aj = aj;
-        smo_pair_update(ai, aj, yi, yj, QDi, QDj, (double)Q[pmi * 64 + pmj], Gi, Gj, C);
+        smo_pair_update(ai, aj, yi, yj, QDi, QDj, (double)Qi[pmj], Gi, Gj, C);
         const double dai = ai - old_ai, daj = aj - old_aj;
-        const bool ui = old_ai >= C, uj = old_aj >= C, ui2 = ai >= C, uj2 = aj >= C;
+        const bool ui = old_ai >= C, uj = old_aj >= C, ui2 = ai >= C, uj2 = aj >= C;   // G_bar's bound changes
 #pragma unroll
         for (int s = 0; s < 2; s++) {
             const int k = lane + 32 * s;
             if (k >= n) continue;
-            const double qi = (double)Q[pmi * 64 + pm[s]], qj = (double)Q[pmj * 64 + pm[s]];
+            const double qi = (double)Qi[own_index(s)], qj = (double)Qj[own_index(s)];
+            // G[k] += Q_i[k]*dai + Q_j[k]*daj, no FMA contraction (as the reference compiles it)
             if (k < active) G[s] = __dadd_rn(G[s], __dadd_rn(__dmul_rn(qi, dai), __dmul_rn(qj, daj)));
-            if (ui != ui2) Gb[s] = ui ? __dsub_rn(Gb[s], __dmul_rn(C, qi)) : __dadd_rn(Gb[s], __dmul_rn(C, qi));
-            if (uj != uj2) Gb[s] = uj ? __dsub_rn(Gb[s], __dmul_rn(C, qj)) : __dadd_rn(Gb[s], __dmul_rn(C, qj));
+            if constexpr (SHRINK) {
+                if (ui != ui2) Gb[s] = ui ? __dsub_rn(Gb[s], __dmul_rn(C, qi)) : __dadd_rn(Gb[s], __dmul_rn(C, qi));
+                if (uj != uj2) Gb[s] = uj ? __dsub_rn(Gb[s], __dmul_rn(C, qj)) : __dadd_rn(Gb[s], __dmul_rn(C, qj));
+            }
             if (k == i) alpha[s] = ai;
             if (k == j) alpha[s] = aj;
         }
     }
-#undef AT
 
     // ---- rho (calculate_rho over the active positions: all of them unless max_iter cut the loop)
     const double rho = svm_rho(y, G, alpha, active, C);
 
-    // ---- predict the held-out samples in training order: alpha_k y_k staged by unpermuted index pm in Q's space
+    // ---- predict the held-out samples in training order: Q is no longer read, its space stages alpha_k y_k by
+    // unpermuted index
     double *coef = reinterpret_cast<double *>(Q);
     __syncwarp();
 #pragma unroll
     for (int s = 0; s < 2; s++)
-        if (lane + 32 * s < n) coef[pm[s]] = alpha[s] * y[s];
+        if (lane + 32 * s < n) coef[own_index(s)] = alpha[s] * y[s];
     __syncwarp();
     int ok;
     unsigned long long bits;
@@ -4048,15 +3930,9 @@ static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int
     CUDA_TRY(fd_buf.alloc(sizeof(SvmFold) * nfolds, st));
     SvmFold *fd = static_cast<SvmFold *>(fd_buf.p);
     CUDA_TRY(cudaMemcpyAsync(fd, fh, sizeof(SvmFold) * nfolds, cudaMemcpyHostToDevice, st));
-    const long nprob = nv * nfolds;
-    if (shrinking) {
-        const size_t smem = (size_t)4 * 64 * 64 * sizeof(float) + 4 * (4 * 64 * sizeof(double) + 2 * 64 * sizeof(int) + 64);
-        return launch_kernel(k_svm_cv_shrink<KT>, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv_shrink", K_dev, nv,
-                             E, nfolds, fd, C, tol, max_iter, correct_dev, iters_dev, bits_dev, Kpred_dev);
-    }
-    const size_t smem = (size_t)4 * 64 * 64 * sizeof(float);
-    return launch_kernel(k_svm_cv<KT>, (unsigned)cdiv(nprob, 4), 128, smem, st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C,
-                         tol, max_iter, correct_dev, iters_dev, bits_dev, Kpred_dev);
+    return launch_kernel(shrinking ? k_svm_cv<KT, true> : k_svm_cv<KT, false>, (unsigned)cdiv(nv * nfolds, 4), 128,
+                         svm_smem_bytes(shrinking), st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C, tol, max_iter,
+                         correct_dev, iters_dev, bits_dev, Kpred_dev);
 }
 
 // ============================================================================================

@@ -729,32 +729,38 @@ def _max_iter_arg(max_iter):
     return -1 if max_iter is None or max_iter < 0 else int(max_iter)
 
 
+def _svm_cv(solve, kernels, K, labels, num_folds, C, tol, max_iter, shrinking, folds, return_iters):
+    """The body of svm_cv_precomputed and svm_cv_f64 around one call of the batched solver ``solve``
+    (fcma_svm_cv_solve or fcma_svm_cv_solve_f64, whose leading arguments are the kernel pointers ``kernels``; ``K`` is
+    one of those kernels): fold problems, outputs, libsvm's one-vs-one vote for more than two classes, and the mean
+    accuracy per kernel."""
+    nv, E, _ = K.shape
+    if folds is None:
+        folds = make_svm_folds(labels, num_folds)
+    nprob = folds.nproblems
+    two = len(folds.classes) == 2
+    with torch.cuda.device(K.device):
+        iters = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if return_iters else None
+        correct = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if two else None
+        bits = None if two else torch.empty((nv, nprob), dtype=torch.int64, device=K.device)
+        _lib.check(solve(*kernels, nv, E, nprob, ctypes.cast(folds.structs, ctypes.c_void_p), float(C), float(tol),
+                         _max_iter_arg(max_iter), 1 if shrinking else 0, _ptr(correct) if two else None,
+                         _ptr(bits) if not two else None, _ptr(iters) if iters is not None else None, _stream_ptr()))
+        if not two:
+            correct = _ovo_vote(bits, folds)
+    scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]   # accuracy_score per fold
+    acc = scores.mean(axis=1)                                                   # cross_val_score(...).mean()
+    return (acc, iters.cpu().numpy()) if return_iters else acc
+
+
 def svm_cv_precomputed(K, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, folds=None, return_iters=False,
                        shrinking=False):
     """Mean cross-validation accuracy of ``SVC(kernel='precomputed', C, tol, shrinking)`` for every kernel of
     ``K`` (float32 CUDA ``[nv, E, E]``), computed by the batched GPU SMO solver.  Equivalent to
     ``cross_val_score(clf, K[v], y=labels, cv=StratifiedKFold(num_folds)).mean()`` per voxel; more than two classes are
     handled one-vs-one with libsvm's vote; ``shrinking`` selects the restatement of libsvm's shrinking heuristic."""
-    lib = _lib.load()
-    nv, E, _ = K.shape
-    if folds is None:
-        folds = make_svm_folds(labels, num_folds)
-    nprob = folds.nproblems
-    cap = _max_iter_arg(max_iter)
-    iters = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if return_iters else None
-    two = len(folds.classes) == 2
-    with torch.cuda.device(K.device):
-        correct = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if two else None
-        bits = None if two else torch.empty((nv, nprob), dtype=torch.int64, device=K.device)
-        _lib.check(lib.fcma_svm_cv_solve(_ptr(K), nv, E, nprob, ctypes.cast(folds.structs, ctypes.c_void_p),
-                                         float(C), float(tol), cap, 1 if shrinking else 0,
-                                         _ptr(correct) if two else None, _ptr(bits) if not two else None,
-                                         _ptr(iters) if iters is not None else None, _stream_ptr()))
-        if not two:
-            correct = _ovo_vote(bits, folds)
-    scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]   # accuracy_score per fold
-    acc = scores.mean(axis=1)                                                   # cross_val_score(...).mean()
-    return (acc, iters.cpu().numpy()) if return_iters else acc
+    return _svm_cv(_lib.load().fcma_svm_cv_solve, (_ptr(K),), K, labels, num_folds, C, tol, max_iter, shrinking, folds,
+                   return_iters)
 
 
 def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, shrinking=True, folds=None,
@@ -769,26 +775,8 @@ def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, s
         raise ValueError("K_fit and K_pred must be float64 [nv, E, E] of the same shape")
     if not (K_fit.is_contiguous() and K_pred.is_contiguous()):
         raise ValueError("K_fit and K_pred must be contiguous")
-    nv, E, _ = K_fit.shape
-    if folds is None:
-        folds = make_svm_folds(labels, num_folds)
-    nprob = folds.nproblems
-    cap = _max_iter_arg(max_iter)
-    two = len(folds.classes) == 2
-    with torch.cuda.device(K_fit.device):
-        iters = torch.empty((nv, nprob), dtype=torch.int32, device=K_fit.device) if return_iters else None
-        correct = torch.empty((nv, nprob), dtype=torch.int32, device=K_fit.device) if two else None
-        bits = None if two else torch.empty((nv, nprob), dtype=torch.int64, device=K_fit.device)
-        _lib.check(lib.fcma_svm_cv_solve_f64(_ptr(K_fit), _ptr(K_pred), nv, E, nprob,
-                                             ctypes.cast(folds.structs, ctypes.c_void_p), float(C), float(tol), cap,
-                                             1 if shrinking else 0, _ptr(correct) if two else None,
-                                             _ptr(bits) if not two else None,
-                                             _ptr(iters) if iters is not None else None, _stream_ptr()))
-        if not two:
-            correct = _ovo_vote(bits, folds)
-    scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]
-    acc = scores.mean(axis=1)
-    return (acc, iters.cpu().numpy()) if return_iters else acc
+    return _svm_cv(lib.fcma_svm_cv_solve_f64, (_ptr(K_fit), _ptr(K_pred)), K_fit, labels, num_folds, C, tol, max_iter,
+                   shrinking, folds, return_iters)
 
 
 # ------------------------------------------------------------------ searchlight (MVPAVoxelSelector)

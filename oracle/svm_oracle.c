@@ -11,8 +11,8 @@
  *
  * Parity status: PINNED against scikit-learn itself -- tests/test_oracle.py requires the iteration count (SVC.n_iter_),
  * rho (intercept_) and the dual coefficients of every problem to equal scikit-learn's, with and without shrinking.
- * The GPU solvers (k_svm_cv, k_svm_cv_shrink) are tested against scikit-learn directly; this file lets the CPU suite
- * check the same restated algorithm without a GPU.
+ * The GPU solver (k_svm_cv, with and without shrinking) is tested against scikit-learn directly; this file lets the CPU
+ * suite check the same restated algorithm without a GPU.
  */
 #include <math.h>
 #include <stdlib.h>

@@ -819,8 +819,8 @@ def test_gpu_svm_cv_matches_sklearn(dev, golden):
 
 def test_gpu_svm_shrinking_follows_libsvm_iteration_by_iteration(dev):
     """libsvm's shrinking heuristic (do_shrinking / be_shrunk / reconstruct_gradient / the counter and unshrink logic of
-    Solver::Solve) restated in k_svm_cv_shrink: on problems that need several hundred iterations -- where variables are
-    shrunk, swapped and the gradient is reconstructed -- the iteration count of EVERY problem equals scikit-learn's
+    Solver::Solve) restated in k_svm_cv<KT, true>: on problems that need several hundred iterations -- where variables
+    are shrunk, swapped and the gradient is reconstructed -- the iteration count of EVERY problem equals scikit-learn's
     SVC.n_iter_ and the accuracies are identical; the counts differ from the unshrunk solver's, i.e. the heuristic ran."""
     from sklearn import model_selection
     rng = RandomState(11)

@@ -1,5 +1,5 @@
-"""Decision-by-decision tests of the batched SVM solver -- ``k_svm_cv`` and ``k_svm_cv_shrink``, each on float and on
-double kernels -- against libsvm itself, as scikit-learn runs it.
+"""Decision-by-decision tests of the batched SVM solver -- ``k_svm_cv`` without and with shrinking, each on float and
+on double kernels -- against libsvm itself, as scikit-learn runs it.
 
 References and bounds
 ---------------------
@@ -32,8 +32,8 @@ Coverage
 --------
 | instantiation / edge                         | covered by                                                          |
 |----------------------------------------------|---------------------------------------------------------------------|
-| ``k_svm_cv<float>``, ``k_svm_cv<double>``      | every GPU test at ``shrinking`` False                                |
-| ``k_svm_cv_shrink<float>`` / ``<double>``     | every GPU test at ``shrinking`` True                                 |
+| ``k_svm_cv<float, false>`` / ``<double, false>`` | every GPU test at ``shrinking`` False                             |
+| ``k_svm_cv<float, true>`` / ``<double, true>``   | every GPU test at ``shrinking`` True                              |
 | n_train 2, 3, 31, 32, 33, 63, 64; n_pos 1, 31, 32, 33, n_train - 1; n_test 0, 1, 31, 32, 33, 64 (bit 63) | test_shapes_in_one_launch |
 | warps of a block on different shapes, partial last block (nv nproblems = 3 mod 4) | test_shapes_in_one_launch, test_degenerate_kernels |
 | held-out indices that are training indices  | test_shapes_in_one_launch                                          |

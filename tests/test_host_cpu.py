@@ -206,7 +206,7 @@ def test_svm_fold_descriptors_follow_sklearn_splits():
         engine.make_svm_folds([0] * 8, 2)                    # a single class
     clf = svm.SVC(kernel="precomputed", shrinking=False)
     assert engine.svm_cv_supported(clf, [0, 1] * 8, 4, 16)
-    # scikit-learn's default shrinking=True: restated as well (k_svm_cv_shrink); allow_shrinking=False keeps it on the host
+    # scikit-learn's default shrinking=True: restated as well (k_svm_cv<KT, true>); allow_shrinking=False keeps it on host
     assert engine.svm_cv_supported(svm.SVC(kernel="precomputed"), [0, 1] * 8, 4, 16)
     assert not engine.svm_cv_supported(svm.SVC(kernel="precomputed"), [0, 1] * 8, 4, 16, allow_shrinking=False)
     assert engine.svm_cv_supported(clf, [0, 1, 2] * 4, 2, 12)                    # one-vs-one on the GPU

@@ -167,7 +167,7 @@ def _svm_problem(rng, E, T, sig, classes=2):
                                            (64, 30, 0.1, 100.0, 1e-3), (32, 200, 0.3, 0.05, 1e-4)])
 def test_svm_solver_restatement_equals_scikit_learn(E, T, sig, C, tol):
     """a8 (voxelselector.py:41-53 -> scikit-learn's libsvm, a third-party dependency of the reference): the sequential
-    restatement in oracle/svm_oracle.c -- the algorithm the CUDA solvers k_svm_cv / k_svm_cv_shrink implement -- against
+    restatement in oracle/svm_oracle.c -- the algorithm the CUDA solver k_svm_cv implements -- against
     SVC.fit on the same precomputed kernels: iteration count, support set, dual coefficients and offset are IDENTICAL, without
     and with the shrinking heuristic (which demonstrably acts on the longer problems: svm_last_stats)."""
     from sklearn import svm
