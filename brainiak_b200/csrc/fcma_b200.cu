@@ -478,10 +478,8 @@ __device__ __forceinline__ float2 fisher_series2(float2 a, float scale)
 // {cols_hi, cols_lo, rows_hi, rows_lo} of a k-block and feeds all three products.
 //   warpgroup 0   : one elected thread issues the TMA loads into a ring of `stages` stages (full / empty mbarriers)
 //   warpgroups 1-2: wgmma m64n256 into 128 fp32 registers per thread, then the epilogue straight from the fragments
-// The epilogue stores pairs of neighbours: in the [i][j] layout two lanes (l, l ^ 4) swap one value so that each
-// holds two consecutive j of one row; in the transposed [j][i] layout a thread's (b = 0, 1) values already are two
-// consecutive i.  In the fp32 block every store instruction of a warp fills whole 32-byte sectors; in the fp16 block
-// it writes 16 contiguous bytes per row.
+// The tiled block leaves through shared memory and TMA bulk stores (gemm_epilogue); the transposed copies and the
+// strided layout are stored from registers, the transposed [j][i] copy as pairs of consecutive i (a thread's b = 0, 1).
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_MAX_STAGES = 8;
 
@@ -506,37 +504,60 @@ struct GemmParams {
     int t_tj0;                     // column tiles [0, t_tj0) are the diagonal block (same voxels as the rows)
     int sym_diag;                  // 1: inside the diagonal block skip tiles tj < ti; tiles tj > ti are mirrored
                                    //    into `out` as tile (tj, ti)
+    uint32_t staging_off;          // smem offset of the tiled block's staging slots (gemm_epilogue)
     uint32_t bar_off;              // smem offset of the mbarriers
     int e_begin;                   // first epoch of this launch
 };
 
-// scale (+ Fisher-z) of the four accumulators of one n-block of a thread; the series form is taken for the warp's
-// 8 x 16 block when no element exceeds its bound, else every element picks its form by its own value
-__device__ __forceinline__ void epilogue_math4(float (&x)[4], float osc, bool do_fisher)
+// scale (+ Fisher-z) of N accumulators of a thread (N / 4 n-blocks).  The series form is taken for the whole warp block
+// when no element exceeds its bound, else every element picks its form by its own value; both branches give each
+// element the form its own value selects (fisher_series1 is one lane of fisher_series2), so the size of the voted block
+// only sets how many independent chains the series branch has and how many votes the epilogue takes
+template <int N>
+__device__ __forceinline__ void epilogue_math(float (&x)[N], float osc, bool do_fisher)
 {
     if (!do_fisher) {
 #pragma unroll
-        for (int k = 0; k < 4; k++) x[k] = __fmaf_rn(x[k], osc, 0.f);
+        for (int k = 0; k < N; k++) x[k] = __fmaf_rn(x[k], osc, 0.f);
         return;
     }
     float m = 0.f;
 #pragma unroll
-    for (int k = 0; k < 4; k++) m = fmaxf(m, fabsf(x[k]));
+    for (int k = 0; k < N; k++) m = fmaxf(m, fabsf(x[k]));
     if (__any_sync(0xffffffffu, m * osc > FISHER_SERIES_MAX)) {
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
+        for (int k = 0; k < N; k++) {
             const float r = x[k] * osc;
             x[k] = fabsf(r) > FISHER_SERIES_MAX ? fisher_fast(r) : fisher_series1(r);
         }
     } else {
-        const float2 a = fisher_series2(make_float2(x[0], x[1]), osc), b = fisher_series2(make_float2(x[2], x[3]), osc);
-        x[0] = a.x, x[1] = a.y, x[2] = b.x, x[3] = b.y;
+#pragma unroll
+        for (int k = 0; k < N; k += 2) {
+            const float2 a = fisher_series2(make_float2(x[k], x[k + 1]), osc);
+            x[k] = a.x, x[k + 1] = a.y;
+        }
     }
 }
 
+// What the epilogue does.  Only the diagnostic build instantiates the variants other than EPI_FULL (FCMA_GEMM_EPILOGUE,
+// tools/gemm_epilogue_probe.py): EPI_NO_STORE does the math and folds the values into one word per thread, stored only if
+// it takes a value that never occurs, so that the math is kept and no store is issued; EPI_NONE skips the epilogue.
+enum { EPI_FULL = 0, EPI_NO_STORE = 1, EPI_NONE = 2 };
+constexpr uint32_t EPI_NEVER = 0x7fbadbadu;
+
+// The tiled block leaves through shared memory: each consumer warpgroup writes its 64 columns of a 32-row chunk into a
+// staging slot laid out as the TMA box of `tm_out` (128-byte swizzle, see make_gemm_out_map), and one thread of the warpgroup
+// stores the box with cp.async.bulk.tensor while the warps go on with the next chunk or the next tile's MMAs.  Two slots
+// per warpgroup: before the barrier that publishes chunk c, the issuing thread waits until chunk c - 1 has been read, so
+// that chunk c + 1 may overwrite its slot.
+constexpr int GEMM_STAGE_SLOTS = 2;   // per consumer warpgroup
 template <bool HALF_OUT>
-__device__ __forceinline__ void gemm_epilogue(const GemmParams &p, float (&acc)[128], int e, int tj, int ti, int half,
-                                              int cw, int warp4, int lane)
+__host__ __device__ constexpr uint32_t gemm_slot_bytes() { return 32 * 64 * (HALF_OUT ? 2 : 4); }
+
+template <bool HALF_OUT, int EPI>
+__device__ __forceinline__ void gemm_epilogue(const GemmParams &p, const CUtensorMap *tm_out, uint32_t staging,
+                                              int &slot, float (&acc)[128], int e, int tj, int ti, int half, int cw,
+                                              int warp4, int lane)
 {
     const int g = lane >> 2, qd = lane & 3, odd = g & 1;
     const int jl0 = half * 128 + cw * 64 + warp4 * 16 + g;   // j inside the 256 tile of h = 0 (h = 1: + 8)
@@ -549,44 +570,87 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams &p, float (&acc)[
         tbase = p.out_t, toff = (((size_t)(tj - p.t_tj0) * p.tiles_i + ti) * p.E + e) * 65536;
     else if (p.sym_diag && tj > ti && tj < p.t_tj0)
         tbase = p.out, toff = (((size_t)tj * p.tiles_j + ti) * p.E + e) * 65536;
-    const size_t tile_off = (((size_t)ti * p.tiles_j + tj) * p.E + e) * 65536;
+    // staging slot offsets of this thread's stores in the first n-block of a chunk: box [j / EPR][32 rows][EPR j] (EPR
+    // elements per 128-byte row), the 16-byte unit inside the row XORed with (row & 7) as SWIZZLE_128B does.  fp32: one
+    // value per store, soff[h][b] for row 2 qd + b and column j; fp16: the pair of the l ^ 4 swap, soff[h][0] for row
+    // 2 qd + odd and columns j - odd, j - odd + 1
+    constexpr int ESZ = HALF_OUT ? 2 : 4, EPR = 128 / ESZ;
+    uint32_t soff[2][2];
 #pragma unroll
-    for (int n = 0; n < 32; n++) {
-        if (i0 + ((8 * n) & ~31) >= p.nb) break;          // 32-row chunks past the block are not written
-        float x[4] = {acc[4 * n], acc[4 * n + 1], acc[4 * n + 2], acc[4 * n + 3]};
-        epilogue_math4(x, p.out_scale, do_fisher);
-        const int il = 8 * n + 2 * qd;                   // rows il (b = 0) and il + 1 (b = 1)
-        if (p.tiled) {
+    for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const float v0 = x[2 * h], v1 = x[2 * h + 1];
-                const float other = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 4);
-                // even g: (row il; columns j, j + 1), odd g: (row il + 1; columns j - 1, j)
-                const size_t off = tile_off + (size_t)(il + odd) * 256 + (jl0 + 8 * h - odd);
-                const float lo = odd ? other : v0, hi = odd ? v1 : other;
-                if constexpr (HALF_OUT) {
-                    *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(p.out) + off) = __floats2half2_rn(lo, hi);
-                    if (tbase)
-                        *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(tbase) + toff + (size_t)(jl0 + 8 * h) * 256 + il) =
-                            __floats2half2_rn(v0, v1);
-                } else {
-                    // the block is far larger than L2 and is read back only by the next kernel: streaming stores keep
-                    // the operand tiles (re-read by every tile of a column group) in L2
-                    __stcs(reinterpret_cast<float2 *>(p.out + off), make_float2(lo, hi));
-                    if (tbase) __stcs(reinterpret_cast<float2 *>(tbase + toff + (size_t)(jl0 + 8 * h) * 256 + il), make_float2(v0, v1));
+        for (int b = 0; b < 2; b++) {
+            const int rq = 2 * qd + (HALF_OUT ? odd : b), jw = warp4 * 16 + 8 * h + g - (HALF_OUT ? odd : 0);
+            soff[h][b] = (uint32_t)(((jw / EPR) * 32 + rq) * 128 + (((jw % EPR) * ESZ) ^ (rq << 4)));
+        }
+    const bool leader = warp4 == 0 && lane == 0;
+    const uint64_t policy = l2_policy_evict_first();
+    uint32_t sink = 0;
+#pragma unroll
+    for (int c = 0; c < 8; c++) {                        // 32-row chunks: n-blocks 4c .. 4c + 3
+        if (i0 + 32 * c >= p.nb) break;                  // chunks past the block are not written
+        float (&xc)[16] = *reinterpret_cast<float (*)[16]>(acc + 16 * c);   // in place: the next tile starts from 0
+        epilogue_math(xc, p.out_scale, do_fisher);
+        const uint32_t slot_addr = staging + (uint32_t)(cw * GEMM_STAGE_SLOTS + slot) * gemm_slot_bytes<HALF_OUT>();
+#pragma unroll
+        for (int n = 4 * c; n < 4 * c + 4; n++) {
+            const float *x = xc + 4 * (n - 4 * c);
+            const int il = 8 * n + 2 * qd;                   // rows il (b = 0) and il + 1 (b = 1)
+            if (p.tiled) {
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const float v0 = x[2 * h], v1 = x[2 * h + 1];
+                    if constexpr (EPI == EPI_NO_STORE) {
+                        sink ^= __float_as_uint(v0) ^ __float_as_uint(v1);
+                        continue;
+                    }
+                    const uint32_t sa = slot_addr + (uint32_t)(n & 3) * 1024;
+                    if constexpr (HALF_OUT) {
+                        // two lanes (l, l ^ 4) swap one value: even g stores (row il; columns j, j + 1), odd g (row il + 1;
+                        // columns j - 1, j)
+                        const float other = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 4);
+                        const float lo = odd ? other : v0, hi = odd ? v1 : other;
+                        sts32(sa + soff[h][0], pack_half2_rn(lo, hi));
+                        if (tbase)
+                            *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(tbase) + toff + (size_t)(jl0 + 8 * h) * 256 + il) =
+                                __floats2half2_rn(v0, v1);
+                    } else {
+                        sts32(sa + soff[h][0], __float_as_uint(v0));
+                        sts32(sa + soff[h][1], __float_as_uint(v1));
+                        // the block is far larger than L2 and is read back only by the next kernel: streaming stores keep
+                        // the operand tiles (re-read by every tile of a column group) in L2
+                        if (tbase) __stcs(reinterpret_cast<float2 *>(tbase + toff + (size_t)(jl0 + 8 * h) * 256 + il), make_float2(v0, v1));
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const long j = p.col_start + (long)tj * 256 + jl0 + 8 * h;
+                    if constexpr (EPI == EPI_NO_STORE) {
+                        sink ^= __float_as_uint(x[2 * h]) ^ __float_as_uint(x[2 * h + 1]);
+                        continue;
+                    }
+                    if (j >= p.V2) continue;
+                    float *ptr = p.out + (size_t)e * p.stride_e + j + (size_t)(i0 + il) * p.stride_i;
+                    if (i0 + il < p.nb) ptr[0] = x[2 * h];
+                    if (i0 + il + 1 < p.nb) ptr[p.stride_i] = x[2 * h + 1];
                 }
             }
-        } else {
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const long j = p.col_start + (long)tj * 256 + jl0 + 8 * h;
-                if (j >= p.V2) continue;
-                float *ptr = p.out + (size_t)e * p.stride_e + j + (size_t)(i0 + il) * p.stride_i;
-                if (i0 + il < p.nb) ptr[0] = x[2 * h];
-                if (i0 + il + 1 < p.nb) ptr[p.stride_i] = x[2 * h + 1];
+        }
+        if (EPI == EPI_FULL && p.tiled) {
+            fence_proxy_async_smem();                        // this thread's staging stores -> the TMA engine
+            if (leader) bulk_wait_read<0>();                 // the previous chunk has left the other slot
+            named_bar_sync(1 + cw, 128);
+            if (leader) {
+                // evict-first in L2, as the register path's st.global.cs: the operand tiles stay
+                tma_store_4d(tm_out, slot_addr, 0, 32 * c, (half * 128 + cw * 64) / EPR, (ti * p.tiles_j + tj) * p.E + e,
+                             policy);
+                bulk_commit();
             }
+            slot ^= 1;
         }
     }
+    if (EPI == EPI_NO_STORE && sink == EPI_NEVER) p.out[0] = 0.f;
 }
 
 template <int FMT>
@@ -628,10 +692,10 @@ __device__ __forceinline__ bool gemm_tile_coords(const GemmParams &p, long tile,
     return !(p.sym_diag && tj < ti);
 }
 
-template <int FMT, int PLANES, bool HALF_OUT>
+template <int FMT, int PLANES, bool HALF_OUT, int EPI = EPI_FULL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     k_corr_wgmma(const __grid_constant__ CUtensorMap tm_cols, const __grid_constant__ CUtensorMap tm_rows,
-                 const GemmParams p)
+                 const __grid_constant__ CUtensorMap tm_out, const GemmParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -688,7 +752,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         setmaxnreg_inc<232>();
         const int cw = wg - 1;             // consumer warpgroup: columns 64 cw .. of the CTA's 128
         const uint32_t tiles_addr = smem_u32(smem);
-        int stage = 0;
+        int stage = 0, slot = 0;
         uint32_t phase = 0;
         float acc[128];
 #pragma unroll
@@ -715,8 +779,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                     phase ^= 1;
                 }
             }
-            gemm_epilogue<HALF_OUT>(p, acc, e, tj, ti, half, cw, warp & 3, lane);
+            if constexpr (EPI != EPI_NONE)
+                gemm_epilogue<HALF_OUT, EPI>(p, &tm_out, tiles_addr + p.staging_off, slot, acc, e, tj, ti, half, cw, warp & 3,
+                                             lane);
         }
+        // the staging slots must stay allocated, and the block written, until the last stores complete
+        if ((warp & 3) == 0 && lane == 0) bulk_wait_all();
     }
 }
 
@@ -761,6 +829,24 @@ static int make_operand_map(CUtensorMap *m, const void *base, const PrecInfo &pi
     return FCMA_OK;
 }
 
+// the GEMM's tiled block [tiles][256 i][256 j] (fp32 or fp16; tiles = tiles_i * tiles_j * E) as the 4-D tensor
+// (j % EPR, i, j / EPR, tile) with EPR = 128 B / element size, so that one box {EPR, 32, 64 / EPR, 1} is a consumer
+// warpgroup's 64 columns of a 32-row chunk in 128-byte rows that SWIZZLE_128B can permute (gemm_epilogue)
+static int make_gemm_out_map(CUtensorMap *m, void *base, size_t tiles, int half_out)
+{
+    PFN_tmEncodeTiled enc = get_encode_fn();
+    if (!enc) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled entry point not available");
+    const cuuint64_t esz = half_out ? 2 : 4, epr = 128 / esz;
+    cuuint64_t gdim[4] = {epr, 256, 256 / epr, (cuuint64_t)tiles};
+    cuuint64_t gstr[3] = {256 * esz, 128, 65536 * esz};
+    cuuint32_t box[4] = {(cuuint32_t)epr, 32, (cuuint32_t)(64 / epr), 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(m, half_out ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, gdim, gstr,
+                     box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled (GEMM block) failed with CUresult %d", (int)r);
+    return FCMA_OK;
+}
 
 // tiled block [ntg tile groups][E][256 i][256 j] (fp32 or fp16) as the 5-D tensor the TMA column pass reads:
 // (j, i%4, tile group * E/4 + e/4, (i%256)/4, e%4), box = one brick (32, 4, 8, 4, 4); see k_norm_syrk_cols_tma
@@ -851,7 +937,9 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     q.tiled = tiled_t256 > 0 ? (half_out ? 2 : 1) : 0;
     if (half_out && !q.tiled) return fail(FCMA_EINVAL, "internal: fp16 output needs the tiled layout");
     if (q.tiled && tiled_t256 != q.tiles_j) return fail(FCMA_EINVAL, "internal: tiled output needs T256 == tiles_j");
-    const size_t cap = 227 * 1024 - 1024 /*alignment slack*/ - 256 /*barriers*/;
+    const uint32_t staging = q.tiled ? 2 * GEMM_STAGE_SLOTS * (half_out ? gemm_slot_bytes<true>() : gemm_slot_bytes<false>())
+                                     : 0;   // two consumer warpgroups
+    const size_t cap = 227 * 1024 - 1024 /*alignment slack*/ - 256 /*barriers*/ - staging;
     int stages = (int)(cap / q.stage_bytes);
     if (stages > GEMM_MAX_STAGES) stages = GEMM_MAX_STAGES;
     {
@@ -860,14 +948,21 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     }
     if (stages < 2) return fail(FCMA_EINVAL, "internal: not enough shared memory for 2 stages");
     q.stages = stages;
-    q.bar_off = (uint32_t)((size_t)stages * q.stage_bytes);
-    const size_t smem = (size_t)stages * q.stage_bytes + 1024 + 256;
+    q.staging_off = (uint32_t)((size_t)stages * q.stage_bytes);   // a multiple of 1024 B, as the swizzle needs
+    q.bar_off = q.staging_off + staging;
+    const size_t smem = (size_t)q.bar_off + 1024 + 256;
 
-    CUtensorMap tm_cols, tm_rows;
+    CUtensorMap tm_cols, tm_rows, tm_out;
     int rc = make_operand_map(&tm_cols, cols_op, pi, E, V2, Kp, 128);
     if (rc) return rc;
     rc = make_operand_map(&tm_rows, rows_op, pi, E, V, Kp, 256);
     if (rc) return rc;
+    memset(&tm_out, 0, sizeof(tm_out));      // the strided layout is stored from registers
+    if (q.tiled) {
+        if ((uintptr_t)out & 15) return fail(FCMA_EINVAL, "internal: the tiled block must be 16-byte aligned");
+        rc = make_gemm_out_map(&tm_out, out, (size_t)q.tiles_i * q.tiles_j * E, half_out);
+        if (rc) return rc;
+    }
 
     // persistent grid: two CTAs (the two column halves) per 256 x 256 tile, one CTA per SM
     long pairs = g_sm_count / 2;
@@ -879,13 +974,28 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
         if (gp && atoi(gp) >= 1 && atoi(gp) < pairs) pairs = atoi(gp);
     }
     auto gemm = [&](auto kernel) {
-        rc = launch_kernel(kernel, (unsigned)(2 * pairs), GEMM_THREADS, smem, st, "k_corr_wgmma", tm_cols, tm_rows, q);
+        rc = launch_kernel(kernel, (unsigned)(2 * pairs), GEMM_THREADS, smem, st, "k_corr_wgmma", tm_cols, tm_rows, tm_out, q);
     };
     // the kernel compiles the product order in (corr_batch): one product with one plane, prec_info's three with two
     const bool order_ok = pi.planes == 1 ? pi.segs == 1
                                          : pi.segs == 3 && pi.seg_r[0] == 1 && pi.seg_r[1] == 0 && pi.seg_r[2] == 0 &&
                                                pi.seg_c[0] == 0 && pi.seg_c[1] == 1 && pi.seg_c[2] == 0;
     auto go = [&](auto FMT, auto PLANES) {
+#ifdef FCMA_DIAG
+        // A/B: FCMA_GEMM_EPILOGUE=1 does the epilogue math without stores, 2 skips the epilogue (results are garbage)
+        const char *ge = diag_env("FCMA_GEMM_EPILOGUE");
+        const int epi = ge ? atoi(ge) : EPI_FULL;
+        if (epi == EPI_NO_STORE) {
+            half_out ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NO_STORE>)
+                     : gemm(k_corr_wgmma<FMT, PLANES, false, EPI_NO_STORE>);
+            return;
+        }
+        if (epi == EPI_NONE) {
+            half_out ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NONE>)
+                     : gemm(k_corr_wgmma<FMT, PLANES, false, EPI_NONE>);
+            return;
+        }
+#endif
         half_out ? gemm(k_corr_wgmma<FMT, PLANES, true>) : gemm(k_corr_wgmma<FMT, PLANES, false>);
     };
     if (!order_ok) return fail(FCMA_EINVAL, "internal: k_corr_wgmma has no product order for precision %d", precision);

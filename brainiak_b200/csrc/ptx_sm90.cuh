@@ -102,6 +102,44 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap *m, uint64_t *bar,
         : "memory");
 }
 
+// L2 policy of a stream written once and read back only after it has left L2 (what st.global.cs asks for)
+__device__ __forceinline__ uint64_t l2_policy_evict_first()
+{
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+// 4-D tiled store shared -> global in the bulk-async group of the issuing thread
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, int c2, int c3,
+                                             uint64_t policy)
+{
+    asm volatile(
+        "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5}], [%1], %6;"
+        :
+        : "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
+        : "memory");
+}
+__device__ __forceinline__ void bulk_commit()
+{
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+// the issuing thread's bulk groups have finished reading shared memory (all but the newest N)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read()
+{
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// the issuing thread's bulk groups have completed (their writes are done)
+__device__ __forceinline__ void bulk_wait_all()
+{
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+// barrier `id` (1..15) of `n` threads, whole warps
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n)
+{
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
 // shared-memory matrix descriptor: K-major tile, 128-byte swizzle, rows of exactly 128 bytes.
 //   start address >> 4 | LBO (unused for swizzled K-major, 1 by convention) | SBO = 8 rows * 128 B = 1024 B |
@@ -286,6 +324,10 @@ __device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], uint32_t a0, uint
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d)
 {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t a)
+{
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(a) : "memory");
 }
 __device__ __forceinline__ uint4 lds128(uint32_t saddr)
 {
