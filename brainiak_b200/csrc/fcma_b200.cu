@@ -829,39 +829,83 @@ static int make_operand_map(CUtensorMap *m, const void *base, const PrecInfo &pi
     return FCMA_OK;
 }
 
-// the GEMM's tiled block [tiles][256 i][256 j] (fp32 or fp16; tiles = tiles_i * tiles_j * E) as the 4-D tensor
+// The correlation block r(i, e, j): `rows` voxel rows x `cols` column voxels x E epochs, written by the GEMM and read by
+// the normalise + kernel-matrix stages (DESIGN.md §2).  Two layouts:
+//   tiled    [ceil(rows/256)][T256][E][256 i][256 j], T256 = ceil(cols/256), fp32 or fp16: every 256 x 256 tile of one
+//            epoch is one contiguous run and the E tiles of one (row block, column block) are adjacent, so row i is read
+//            as E runs of 256 elements per column tile.  The fused pipelines' work buffer.
+//   strided  fp32 only, element (i, e, j) at i*stride_i + e*stride_e + j: the caller's buffer of fcma_corr_block and of
+//            the kernel-matrix entry points, and run_pipeline's block when it cannot be tiled.
+// The kernels take both as (stride_i, ld, chunk_step): element (i, e, j) at i*stride_i + e*ld + (j/256)*chunk_step + j%256
+// (strided: chunk_step = 256), where a tiled block counts i inside its 256-row block and the 256-row blocks lie
+// rb_stride() elements apart.  A column range of a tiled block keeps its parent's T256, and so its row-block stride.
+struct CorrBlock {
+    void *base = nullptr;          // nullptr: no block
+    int E = 0;
+    long rows = 0, cols = 0;
+    bool tiled = false, fp16 = false;
+    long stride_i = 0, ld = 0, chunk_step = 256;
+    long t256 = 0;                 // column tiles per 256-row block
+    int rc = FCMA_OK;              // FCMA_EINVAL when the block breaks a layout invariant; every launcher returns it
+
+    CorrBlock() = default;
+    CorrBlock(const float *p, int E_, long rows_, long cols_, long stride_i_, long stride_e)
+        : base(const_cast<float *>(p)), E(E_), rows(rows_), cols(cols_), stride_i(stride_i_), ld(stride_e),
+          t256(cdiv(cols_, 256)) {}
+    CorrBlock(void *p, int E_, long rows_, long cols_, bool fp16_)
+        : base(p), E(E_), rows(rows_), cols(cols_), tiled(true), fp16(fp16_), stride_i(256), ld(65536),
+          chunk_step((long)E_ * 65536), t256(cdiv(cols_, 256))
+    {
+        if ((uintptr_t)p & 15) rc = fail(FCMA_EINVAL, "internal: the tiled block must be 16-byte aligned");
+    }
+    size_t esz() const { return fp16 ? sizeof(__half) : sizeof(float); }
+    long rb_stride() const { return tiled ? t256 * chunk_step : 0; }
+    // bytes of a tiled block (0 for a strided block or none); end(): where the next tiled block of the work buffer starts
+    size_t bytes() const { return (size_t)cdiv(rows, 256) * rb_stride() * esz(); }
+    void *end() const { return static_cast<uint8_t *>(base) + bytes(); }
+    // columns [c0, c1) of a tiled block; c0 starts a column tile
+    CorrBlock columns(long c0, long c1) const
+    {
+        CorrBlock r = *this;
+        r.base = static_cast<uint8_t *>(base) + (size_t)(c0 / 256) * chunk_step * esz(), r.cols = c1 - c0;
+        if (!tiled || (c0 & 255)) r.rc = fail(FCMA_EINVAL, "internal: a column range of the tiled block starts at a tile");
+        return r;
+    }
+};
+
+// the GEMM's tiled block as [tiles][256 i][256 j] (tiles = ceil(rows/256) * T256 * E), the 4-D tensor
 // (j % EPR, i, j / EPR, tile) with EPR = 128 B / element size, so that one box {EPR, 32, 64 / EPR, 1} is a consumer
 // warpgroup's 64 columns of a 32-row chunk in 128-byte rows that SWIZZLE_128B can permute (gemm_epilogue)
-static int make_gemm_out_map(CUtensorMap *m, void *base, size_t tiles, int half_out)
+static int make_gemm_out_map(CUtensorMap *m, const CorrBlock &out)
 {
     PFN_tmEncodeTiled enc = get_encode_fn();
     if (!enc) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-    const cuuint64_t esz = half_out ? 2 : 4, epr = 128 / esz;
-    cuuint64_t gdim[4] = {epr, 256, 256 / epr, (cuuint64_t)tiles};
-    cuuint64_t gstr[3] = {256 * esz, 128, 65536 * esz};
+    const cuuint64_t esz = out.esz(), epr = 128 / esz;
+    cuuint64_t gdim[4] = {epr, 256, 256 / epr, (cuuint64_t)(cdiv(out.rows, 256) * out.t256 * out.E)};
+    cuuint64_t gstr[3] = {256 * esz, 128, out.ld * esz};
     cuuint32_t box[4] = {(cuuint32_t)epr, 32, (cuuint32_t)(64 / epr), 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, half_out ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, gdim, gstr,
-                     box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = enc(m, out.fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.base, gdim,
+                     gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled (GEMM block) failed with CUresult %d", (int)r);
     return FCMA_OK;
 }
 
-// tiled block [ntg tile groups][E][256 i][256 j] (fp32 or fp16) as the 5-D tensor the TMA column pass reads:
-// (j, i%4, tile group * E/4 + e/4, (i%256)/4, e%4), box = one brick (32, 4, 8, 4, 4); see k_norm_syrk_cols_tma
-static int make_cols_map(CUtensorMap *m, const void *base, size_t ntg, int E, int half_in)
+// tiled block as [ntg tile groups][E][256 i][256 j] (ntg = ceil(rows/256) * T256), the 5-D tensor the TMA column pass
+// reads: (j, i%4, tile group * E/4 + e/4, (i%256)/4, e%4), box = one brick (32, 4, 8, 4, 4); see k_norm_syrk_cols_tma
+static int make_cols_map(CUtensorMap *m, const CorrBlock &A)
 {
     PFN_tmEncodeTiled enc = get_encode_fn();
     if (!enc) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-    const cuuint64_t esz = half_in ? 2 : 4;
-    cuuint64_t gdim[5] = {256, 4, (cuuint64_t)ntg * (cuuint64_t)(E / 4), 64, 4};
-    cuuint64_t gstr[4] = {256 * esz, 4 * 65536 * esz, 4 * 256 * esz, 65536 * esz};
+    const cuuint64_t esz = A.esz();
+    cuuint64_t gdim[5] = {256, 4, (cuuint64_t)(cdiv(A.rows, 256) * A.t256) * (cuuint64_t)(A.E / 4), 64, 4};
+    cuuint64_t gstr[4] = {256 * esz, 4 * A.ld * esz, 4 * 256 * esz, A.ld * esz};
     cuuint32_t box[5] = {32, 4, 8, 4, 4};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(m, half_in ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5,
-                     const_cast<void *>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     half_in ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+    CUresult r = enc(m, A.fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, A.base, gdim, gstr,
+                     box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     A.fp16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(FCMA_ECUDA, "cuTensorMapEncodeTiled (column pass) failed with CUresult %d", (int)r);
     return FCMA_OK;
@@ -890,20 +934,19 @@ __global__ void k_self_corr_fixup(const float *__restrict__ selfdiag, int E, lon
     }
 }
 
-// tiled_t256 > 0: write the block in the tiled layout [ceil(nb/256)][tiled_t256][E][256][256] (the caller
-// provides round_up(nb, 256) rows of workspace and tiled_t256 == ceil(V2/256)); else out[i*stride_i + e*stride_e + j]
-// Symmetric mode (sym != nullptr; self-correlation, tiled fp32 output): the block covers columns [col_start, V2)
+// Rows [start, start + out.rows) x columns [0, V2) into `out`; a tiled block holds round_up(rows, 256) rows.
+// Symmetric mode (sym != nullptr; self-correlation, tiled output): the block covers columns [col_start, V2)
 // with col_start == start; column tiles below t_tj0 = ceil(nb/256) are the diagonal block, where only tiles
 // tj >= ti are computed and tiles tj > ti are mirrored into `out`; every tile with tj >= t_tj0 is also stored
-// transposed into sym->out_t, a tiled block [tiles_j - t_tj0][ceil(nb/256)][E][256][256] (rows = the column voxels).
-struct SymOut {
-    float *out_t;      // nullptr: no transposed block (the column-direction pass reads block A instead)
-};
-static int launch_corr_mma(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2,
-                           long start, long nb, float *out, long stride_i, long stride_e, int fisher_epochs,
-                           cudaStream_t st, long tiled_t256 = 0, int half_out = 0, const SymOut *sym = nullptr,
+// transposed into *sym, block B: rows [start + nb, V) x columns [start, start + nb) (CorrBlock(): none, when the
+// column-direction pass reads `out` instead).
+static int launch_corr_mma(const void *rows_op, const void *cols_op, int precision, int T, long V, long V2, long start,
+                           const CorrBlock &out, int fisher_epochs, cudaStream_t st, const CorrBlock *sym = nullptr,
                            int e_begin = 0, int e_count = -1, bool fixup = true)
 {
+    const int E = out.E;
+    const long nb = out.rows;
+    if (out.rc) return out.rc;
     PrecInfo pi;
     if (!prec_info(precision, &pi)) return fail(FCMA_EINVAL, "unknown precision %d", precision);
     if (E <= 0 || T <= 0 || V <= 0 || V2 <= 0 || nb <= 0 || start < 0 || start + nb > V)
@@ -921,23 +964,24 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     q.col_start = sym ? start : 0;
     q.tiles_j = (int)cdiv(V2 - q.col_start, 256), q.tiles_i = (int)cdiv(nb, 256);
     if (sym) {
-        if (rows_op != cols_op || V != V2 || tiled_t256 <= 0 || ((nb & 255) && start + nb != V))
+        if (sym->rc) return sym->rc;
+        if (rows_op != cols_op || V != V2 || !out.tiled || ((nb & 255) && start + nb != V))
             return fail(FCMA_EINVAL, "internal: symmetric GEMM needs self-correlation, the tiled block and whole row tiles");
         q.sym_diag = 1;
         q.t_tj0 = q.tiles_i;
-        q.out_t = q.tiles_j > q.tiles_i ? sym->out_t : nullptr;
+        q.out_t = q.tiles_j > q.tiles_i ? static_cast<float *>(sym->base) : nullptr;
     }
     if (e_count < 0) e_count = E - e_begin;
     if (e_begin < 0 || e_count <= 0 || e_begin + e_count > E) return fail(FCMA_EINVAL, "internal: bad epoch range [%d, +%d) of %d", e_begin, e_count, E);
     q.e_begin = e_begin;
     q.total_tiles = (long)q.tiles_j * q.tiles_i * e_count;
-    q.out = out, q.stride_i = stride_i, q.stride_e = stride_e, q.fisher_epochs = fisher_epochs;
+    // a tiled block is stored through TMA and never read through the strides (gemm_epilogue, k_self_corr_fixup)
+    q.out = static_cast<float *>(out.base), q.stride_i = out.stride_i, q.stride_e = out.ld, q.fisher_epochs = fisher_epochs;
     q.out_scale = 1.0f / (pi.in_scale * pi.in_scale);
     q.stage_bytes = (uint32_t)pi.planes * (16384 + 32768);
-    q.tiled = tiled_t256 > 0 ? (half_out ? 2 : 1) : 0;
-    if (half_out && !q.tiled) return fail(FCMA_EINVAL, "internal: fp16 output needs the tiled layout");
-    if (q.tiled && tiled_t256 != q.tiles_j) return fail(FCMA_EINVAL, "internal: tiled output needs T256 == tiles_j");
-    const uint32_t staging = q.tiled ? 2 * GEMM_STAGE_SLOTS * (half_out ? gemm_slot_bytes<true>() : gemm_slot_bytes<false>())
+    q.tiled = out.tiled ? (out.fp16 ? 2 : 1) : 0;
+    if (q.tiled && out.t256 != q.tiles_j) return fail(FCMA_EINVAL, "internal: tiled output needs T256 == tiles_j");
+    const uint32_t staging = q.tiled ? 2 * GEMM_STAGE_SLOTS * (out.fp16 ? gemm_slot_bytes<true>() : gemm_slot_bytes<false>())
                                      : 0;   // two consumer warpgroups
     const size_t cap = 227 * 1024 - 1024 /*alignment slack*/ - 256 /*barriers*/ - staging;
     int stages = (int)(cap / q.stage_bytes);
@@ -958,11 +1002,7 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
     rc = make_operand_map(&tm_rows, rows_op, pi, E, V, Kp, 256);
     if (rc) return rc;
     memset(&tm_out, 0, sizeof(tm_out));      // the strided layout is stored from registers
-    if (q.tiled) {
-        if ((uintptr_t)out & 15) return fail(FCMA_EINVAL, "internal: the tiled block must be 16-byte aligned");
-        rc = make_gemm_out_map(&tm_out, out, (size_t)q.tiles_i * q.tiles_j * E, half_out);
-        if (rc) return rc;
-    }
+    if (q.tiled && (rc = make_gemm_out_map(&tm_out, out))) return rc;
 
     // persistent grid: two CTAs (the two column halves) per 256 x 256 tile, one CTA per SM
     long pairs = g_sm_count / 2;
@@ -986,17 +1026,17 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
         const char *ge = diag_env("FCMA_GEMM_EPILOGUE");
         const int epi = ge ? atoi(ge) : EPI_FULL;
         if (epi == EPI_NO_STORE) {
-            half_out ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NO_STORE>)
+            out.fp16 ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NO_STORE>)
                      : gemm(k_corr_wgmma<FMT, PLANES, false, EPI_NO_STORE>);
             return;
         }
         if (epi == EPI_NONE) {
-            half_out ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NONE>)
+            out.fp16 ? gemm(k_corr_wgmma<FMT, PLANES, true, EPI_NONE>)
                      : gemm(k_corr_wgmma<FMT, PLANES, false, EPI_NONE>);
             return;
         }
 #endif
-        half_out ? gemm(k_corr_wgmma<FMT, PLANES, true>) : gemm(k_corr_wgmma<FMT, PLANES, false>);
+        out.fp16 ? gemm(k_corr_wgmma<FMT, PLANES, true>) : gemm(k_corr_wgmma<FMT, PLANES, false>);
     };
     if (!order_ok) return fail(FCMA_EINVAL, "internal: k_corr_wgmma has no product order for precision %d", precision);
     if (pi.fmt == 0 && pi.planes == 2) go(IntC<0>{}, IntC<2>{});        // fp16x3
@@ -1012,8 +1052,8 @@ static int launch_corr_mma(const void *rows_op, const void *cols_op, int precisi
         const float *sd = reinterpret_cast<const float *>(reinterpret_cast<const uint8_t *>(rows_op) +
                                                           operand_plane_bytes(pi, precision, E, T, V));
         long n = nb * E;
-        k_self_corr_fixup<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(sd, E, V, start, nb, out, stride_i, stride_e,
-                                                                 fisher_epochs, tiled_t256, half_out, q.col_start);
+        k_self_corr_fixup<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(sd, E, V, start, nb, q.out, out.stride_i, out.ld,
+                                                                 fisher_epochs, out.tiled ? out.t256 : 0, out.fp16, q.col_start);
         LAUNCH_CHECK("k_self_corr_fixup");
     }
     return FCMA_OK;
@@ -2613,29 +2653,24 @@ static bool fused_supported(int E, int eps_mode)
     return eps_mode <= (E <= 32 ? 32 : 64);
 }
 
-// (stride_i, ld, chunk_step) describe where element (i, e, j) of the correlation block lives:
-//   C[i*stride_i + e*ld + (j/256)*chunk_step + j%256]
-// classic [nb][E][ld] layout: stride_i = E*ld, chunk_step = 256.  Tiled [nb/256][T256][E][256 i][256 j] layout
-// (every 256x256 pair tile of the GEMM is one contiguous 256 KB run; the E tiles of one (row block, column
-// block) are adjacent): stride_i = 256, ld = 65536, chunk_step = E*65536, and i -> (i/256)*T256*chunk_step +
-// (i%256)*stride_i inside the kernel.
-// rb_stride: elements between 256-row blocks of a tiled block when the kernel is given only a column RANGE of it (0: the
-// range is the whole block); K64: optional fp64 accumulator [E][E] for sum_over_rows (then K is not touched)
-static int launch_norm_syrk(const float *C, long nb, int E, long n2, long stride_i, long ld, int eps_mode,
-                            int fisher_done, long self_col0, float beta, float *K, int sum_over_rows, cudaStream_t st,
-                            long chunk_step = 256, int half_in = 0, long rb_stride = 0, double *K64 = nullptr)
+// K[i] of the block's rows i (sum_over_rows: their sum into K); K64: optional fp64 accumulator [E][E] for sum_over_rows
+// (then K is not touched)
+static int launch_norm_syrk(const CorrBlock &C, int eps_mode, int fisher_done, long self_col0, float beta, float *K,
+                            int sum_over_rows, cudaStream_t st, double *K64 = nullptr)
 {
+    const int E = C.E;
+    const long nb = C.rows;
+    if (C.rc) return C.rc;
     if (!fused_supported(E, eps_mode)) return fail(FCMA_EINVAL, "internal: fused norm+syrk unsupported E=%d eps=%d", E, eps_mode);
     if (sum_over_rows && !K64) {
         // K = beta*K, then atomically accumulate the per-row kernels
         k_scale<<<1, 256, 0, st>>>(K, (long)E * E, beta);
         LAUNCH_CHECK("k_scale");
     }
-    const bool vec = ((ld & 3) == 0) && ((stride_i & 3) == 0) && (((uintptr_t)C & 15) == 0);
-    if (!vec && chunk_step != 256) return fail(FCMA_EINVAL, "internal: tiled layout needs the vector path");
+    // a tiled block is 16-byte aligned, so it always takes the vector path
+    const bool vec = ((C.ld & 3) == 0) && ((C.stride_i & 3) == 0) && (((uintptr_t)C.base & 15) == 0);
     const bool fisher = eps_mode > 0 && !fisher_done;
-    if (half_in && (fisher || chunk_step == 256 || !vec))
-        return fail(FCMA_EINVAL, "internal: the fp16 block is tiled and already Fisher-transformed");
+    if (C.fp16 && fisher) return fail(FCMA_EINVAL, "internal: the fp16 block is tiled and already Fisher-transformed");
     // rows cost the same: a static stride over 16 blocks per SM balances well
     long g = nb < 16L * g_sm_count ? nb : 16L * g_sm_count;
     int rc = FCMA_OK;
@@ -2645,20 +2680,21 @@ static int launch_norm_syrk(const float *C, long nb, int E, long n2, long stride
         constexpr size_t smem = (VEC ? (size_t)8 * 2 * (VEC == 2 ? R : 2 * R) * 32 * sizeof(float4) : 0) +
                                 (R <= 4 ? (size_t)8 * (8 * R) * (8 * R) * sizeof(float) : 0);
         auto go = [&](auto EPS) {
-            rc = launch_kernel(k_norm_syrk<R, EPS, FISHER, VEC>, (unsigned)g, 256, smem, st, "k_norm_syrk", C, nb, E, n2,
-                               stride_i, ld, chunk_step, self_col0, beta, K, sum_over_rows, rb_stride, K64);
+            rc = launch_kernel(k_norm_syrk<R, EPS, FISHER, VEC>, (unsigned)g, 256, smem, st, "k_norm_syrk",
+                               static_cast<const float *>(C.base), nb, E, C.cols, C.stride_i, C.ld, C.chunk_step, self_col0,
+                               beta, K, sum_over_rows, C.rb_stride(), K64);
         };
         if constexpr (R == 2) return with_int<0, 1, 2, 4, 8, 16>(eps_mode, go);
         else if constexpr (R == 4) return with_int<0, 1, 2, 4, 8, 16, 32>(eps_mode, go);
         else return with_int<0, 1, 2, 4, 8, 16, 32, 64>(eps_mode, go);
     };
     auto per_layout = [&](auto R) {   // VEC: 0 scalar loads, 1 cp.async of an fp32 block, 2 of an fp16 block
-        if (half_in) return run(R, std::false_type{}, IntC<2>{});
+        if (C.fp16) return run(R, std::false_type{}, IntC<2>{});
         if (fisher) return vec ? run(R, std::true_type{}, IntC<1>{}) : run(R, std::true_type{}, IntC<0>{});
         return vec ? run(R, std::false_type{}, IntC<1>{}) : run(R, std::false_type{}, IntC<0>{});
     };
     bool ok;
-    if (E <= 16 && eps_mode <= 16 && !half_in && !fisher && vec)
+    if (E <= 16 && eps_mode <= 16 && !C.fp16 && !fisher && vec)
         // 16 padded epochs instead of 32 (lane = 2 epochs): half the statistics and MMA work per byte of the pipelines'
         // fp32 block (BASELINE configs[1]: E = 16)
         ok = run(IntC<2>{}, std::false_type{}, IntC<1>{});
@@ -2668,16 +2704,22 @@ static int launch_norm_syrk(const float *C, long nb, int E, long n2, long stride
     return rc;
 }
 
-// column-direction pass over a tiled fp32 block (k_norm_syrk_cols): K[j] += ... for block columns [c0, n2)
+// column-direction pass over a tiled block (k_norm_syrk_cols): K[j] += ... for block columns [c0, cols); `flags` picks
+// the opt-in variants (FCMA_FLAG_COLS_*)
 static bool cols_supported(int E, int eps)
 {
     return E <= 64 && eps >= 1 && eps <= (E <= 32 ? 32 : 64) && (eps & (eps - 1)) == 0;
 }
-static int launch_norm_syrk_cols(const void *A, long n, int E, long n2, long T256, long c0, int eps, float *K,
-                                 cudaStream_t st, int half_in = 0, bool use_tma = false, bool v2 = false, bool pad32 = false)
+static int launch_norm_syrk_cols(const CorrBlock &A, long c0, int eps, float *K, cudaStream_t st, int flags)
 {
-    if (!cols_supported(E, eps) || (c0 & 31) || c0 >= n2) return fail(FCMA_EINVAL, "internal: column pass unsupported E=%d eps=%d c0=%ld", E, eps, c0);
-    const float *A32 = reinterpret_cast<const float *>(A);
+    const int E = A.E;
+    const long n = A.rows, n2 = A.cols, T256 = A.t256;
+    const bool half_in = A.fp16, use_tma = (flags & FCMA_FLAG_COLS_TMA) != 0, v2 = (flags & FCMA_FLAG_COLS_V2) != 0,
+               pad32 = (flags & FCMA_FLAG_COLS_PAD32) != 0;
+    if (A.rc) return A.rc;
+    if (!A.tiled || !cols_supported(E, eps) || (c0 & 31) || c0 >= n2)
+        return fail(FCMA_EINVAL, "internal: column pass unsupported E=%d eps=%d c0=%ld", E, eps, c0);
+    const float *A32 = static_cast<const float *>(A.base);
     int rc = FCMA_OK;
     if (E > 32) {   // 32 < E <= 64, fp32 block: one column per warp, 8-column strips (k_norm_syrk_cols64)
         if (half_in) return fail(FCMA_EINVAL, "internal: no column pass over an fp16 block for E=%d", E);
@@ -2695,9 +2737,9 @@ static int launch_norm_syrk_cols(const void *A, long n, int E, long n2, long T25
     // FCMA_FLAG_COLS_TMA: TMA-fed bricks + mbarrier ring (k_norm_syrk_cols_tma) when the block can be described to TMA (E a
     // multiple of 4) and K allows 16-byte read-modify-writes.  It removes the 4096 LDGSTS per brick and the per-brick
     // bar.sync; opt-in, the cp.async kernel below stays the default.
-    if (use_tma && (E & 3) == 0 && ((uintptr_t)K & 15) == 0 && ((uintptr_t)A & 15) == 0) {
+    if (use_tma && (E & 3) == 0 && ((uintptr_t)K & 15) == 0) {
         CUtensorMap tmA;
-        rc = make_cols_map(&tmA, A, (size_t)cdiv(n, 256) * (size_t)T256, E, half_in);
+        rc = make_cols_map(&tmA, A);
         if (rc) return rc;
         const size_t smem_t = 196608 + 64 + 1024;
         auto go = [&](auto kernel) {
@@ -2741,7 +2783,7 @@ static int launch_norm_syrk_cols(const void *A, long n, int E, long n2, long T25
     // bricks (3 x 64 KB fp32 / 3 x 32 KB fp16); the fold buffer [32 columns][32*32] fp32 = 128 KB overlays them
     const size_t smem = (half_in ? (size_t)131072 : (size_t)COLS_BRICKS * 65536) + 1024;
     auto go = [&](auto kernel, unsigned threads) {
-        rc = launch_kernel(kernel, grid, threads, smem, st, "k_norm_syrk_cols", A, n, E, n2, T256, c0, K);
+        rc = launch_kernel(kernel, grid, threads, smem, st, "k_norm_syrk_cols", A.base, n, E, n2, T256, c0, K);
     };
     if (!with_int<1, 2, 4, 8, 16, 32>(eps, [&](auto EPS) {
             if (half_in) return go(k_norm_syrk_cols<EPS, 4, true>, 256);
@@ -2842,8 +2884,8 @@ extern "C" int fcma_corr_block(const void *rows_op, const void *cols_op, int pre
     int rc = check_device();
     if (rc) return rc;
     if (!rows_op || !cols_op || !out_dev) return fail(FCMA_EINVAL, "fcma_corr_block: null pointer");
-    return launch_corr_mma(rows_op, cols_op, precision, E, T, V, V2, start, nb, out_dev, stride_i, stride_e,
-                            fisher_epochs, (cudaStream_t)stream);
+    return launch_corr_mma(rows_op, cols_op, precision, T, V, V2, start, CorrBlock(out_dev, E, nb, V2, stride_i, stride_e),
+                           fisher_epochs, (cudaStream_t)stream);
 }
 
 extern "C" int fcma_corr_block_f32(const float *rows_epochs, long ldr, const float *cols_epochs, long ldc, int E, int T,
@@ -2898,7 +2940,7 @@ extern "C" int fcma_kernel_matrices(const float *z_dev, long nb, int E, long n2,
     if (rc) return rc;
     if (!z_dev || !K_dev || nb <= 0 || E <= 0 || n2 <= 0 || ld < n2) return fail(FCMA_EINVAL, "fcma_kernel_matrices: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    if (fused_supported(E, 0)) return launch_norm_syrk(z_dev, nb, E, n2, stride_i, ld, 0, 1, -1, beta, K_dev, sum_over_rows, st);
+    if (fused_supported(E, 0)) return launch_norm_syrk(CorrBlock(z_dev, E, nb, n2, stride_i, ld), 0, 1, -1, beta, K_dev, sum_over_rows, st);
     return launch_syrk_simt(z_dev, nb, E, n2, stride_i, ld, beta, K_dev, sum_over_rows, st);
 }
 
@@ -2913,8 +2955,8 @@ extern "C" int fcma_norm_kernel_matrices(const float *corr_dev, long nb, int E, 
     if (!fused_supported(E, eps))
         return fail(FCMA_EINVAL, "fused normalise+kernel needs E <= 64 and a power-of-two epochs_per_subj (E=%d eps=%d): "
                                  "use fcma_within_subject_norm + fcma_kernel_matrices", E, eps);
-    return launch_norm_syrk(corr_dev, nb, E, n2, stride_i, ld, eps, fisher_done, self_col0, beta, K_dev, sum_over_rows,
-                            (cudaStream_t)stream);
+    return launch_norm_syrk(CorrBlock(corr_dev, E, nb, n2, stride_i, ld), eps, fisher_done, self_col0, beta, K_dev,
+                            sum_over_rows, (cudaStream_t)stream);
 }
 
 extern "C" size_t fcma_work_bytes_per_row(int E, long V2)
@@ -3009,8 +3051,8 @@ struct FeatureStage {
     double gamma;
     double *K_fit, *K_pred;
 };
-static int launch_norm_gram_f64(const float *C, long nb, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
-                                int eps, int kind, double gamma, double *K_fit, double *K_pred, cudaStream_t st);
+static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
+                                cudaStream_t st);
 
 // shared body of the fused pipelines; with `feat` the GEMM writes raw r and the feature stage replaces normalise+SYRK
 static int run_pipeline(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2, long start,
@@ -3034,25 +3076,18 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
     if (mask_self && (feat || !(normalise && fused)))
         return fail(FCMA_EINVAL, "FCMA_FLAG_MASK_SELF needs the fused normalise+kernel path (E <= 64, power-of-two eps)");
-    // Tiled intermediate [n/256][T256][E][256][256]: every 256x256 pair tile of the GEMM is one contiguous 256 KB
-    // run and the E tiles of one (row block, column block) are adjacent, so the fused normalise+SYRK kernel reads
-    // row i as E runs of 1 KB, 256 KB apart, inside one 8 MB region.  Needs whole 256-row blocks of workspace.
-    // FCMA_FLAG_STRIDED_BLOCK keeps the strided [i][e][j] block.
-    const long t256 = cdiv(V2, 256);
+    // the tiled block (CorrBlock) needs whole 256-row blocks of workspace; FCMA_FLAG_STRIDED_BLOCK keeps the strided
+    // [i][e][ld] block
     const bool tiled = !(flags & FCMA_FLAG_STRIDED_BLOCK) && (fused || feat) && V2 < (1L << 31) && rows_per_pass >= 256;
     // an fp16 block needs the tiled layout and holds Fisher-z values (applied in the GEMM epilogue)
     const bool half16 = half_block(precision, flags) && tiled && normalise && fisher_in_gemm;
     for (long done = 0; done < nb; done += rows_per_pass) {
         const long n = nb - done < rows_per_pass ? nb - done : rows_per_pass;
+        const CorrBlock C = tiled ? CorrBlock(work, E, n, V2, half16) : CorrBlock(work, E, n, V2, (long)E * ld, ld);
         PassTimer timer(st);
         int rc = timer.start();
         if (rc) return rc;
-        if (tiled)
-            rc = launch_corr_mma(rows_op, cols_op, precision, E, T, V, V2, start + done, n, work, 4, 4,
-                                  fisher_in_gemm ? S_eps : 0, st, t256, half16 ? 1 : 0);
-        else
-            rc = launch_corr_mma(rows_op, cols_op, precision, E, T, V, V2, start + done, n, work, (long)E * ld, ld,
-                                  fisher_in_gemm ? S_eps : 0, st);
+        rc = launch_corr_mma(rows_op, cols_op, precision, T, V, V2, start + done, C, fisher_in_gemm ? S_eps : 0, st);
         if (rc) return rc;
         rc = timer.gemm_done();
         if (rc) return rc;
@@ -3060,16 +3095,10 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
         const float beta = sum_over_rows ? 1.0f : 0.0f;
         if (feat) {
             const size_t off = (size_t)done * E * E;
-            rc = tiled ? launch_norm_gram_f64(work, n, E, V2, 256, 65536, (long)E * 65536, t256, eps, feat->kind, feat->gamma,
-                                              feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st)
-                       : launch_norm_gram_f64(work, n, E, V2, (long)E * ld, ld, 256, t256, eps, feat->kind, feat->gamma,
-                                              feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st);
-        } else if (tiled) {
-            rc = launch_norm_syrk(work, n, E, V2, 256, 65536, normalise ? eps : 0, (normalise && fisher_in_gemm) ? 1 : 0,
-                                  mask_self ? start + done : -1, beta, Kdst, sum_over_rows, st, (long)E * 65536,
-                                  half16 ? 1 : 0);
-        } else if (normalise && fused) {
-            rc = launch_norm_syrk(work, n, E, V2, (long)E * ld, ld, eps, fisher_in_gemm ? 1 : 0,
+            rc = launch_norm_gram_f64(C, eps, feat->kind, feat->gamma, feat->K_fit + off,
+                                      feat->K_pred ? feat->K_pred + off : nullptr, st);
+        } else if (tiled || (normalise && fused)) {
+            rc = launch_norm_syrk(C, normalise ? eps : 0, (normalise && fisher_in_gemm) ? 1 : 0,
                                   mask_self ? start + done : -1, beta, Kdst, sum_over_rows, st);
         } else {
             if (normalise) {
@@ -3084,7 +3113,7 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
                 }
             }
             if (fused_supported(E, 0))
-                rc = launch_norm_syrk(work, n, E, V2, (long)E * ld, ld, 0, 1, -1, beta, Kdst, sum_over_rows, st);
+                rc = launch_norm_syrk(C, 0, 1, -1, beta, Kdst, sum_over_rows, st);
             else
                 rc = launch_syrk_simt(work, n, E, V2, (long)E * ld, ld, beta, Kdst, sum_over_rows, st);
         }
@@ -3124,14 +3153,18 @@ extern "C" int fcma_sym_uses_column_pass(int precision, int E, int eps, int flag
     return sym_uses_cols(precision, E, eps, flags) ? 1 : 0;
 }
 
-// Hooks of the host-buffer entry point (fcma_host_voxel_kernels_sym): the first pass' GEMM runs epoch group by epoch group
-// as the groups arrive from the host (a GEMM tile needs only its own epoch), and the kernels of a pass are read back while the
-// next pass computes (K rows [a, a+n) are final once the pass' row kernel has run).
+// Hooks of the grouped entry points (fcma_voxel_kernels_sym_grouped, fcma_host_voxel_kernels_sym): the epochs arrive in
+// groups, and the first pass' GEMM runs epoch group by epoch group, each group packed into `op` (voxels [start, V)) once its
+// event has fired (a GEMM tile needs only its own epoch).  With K_host the kernels of a pass are read back while the next
+// pass computes (K rows [a, a+n) are final once the pass' row kernel has run).
 struct SymHostHooks {
     int ngroups = 0;
     const int *e0 = nullptr, *cnt = nullptr;                  // epoch groups of the upload
-    int (*prepare)(void *ctx, int g, cudaStream_t st) = nullptr;   // make group g's packed operand available on `st`
-    void *ctx = nullptr;
+    const cudaEvent_t *ready = nullptr;                       // per group: its epochs are in `epochs` (null: already there)
+    const float *epochs = nullptr;                            // [E][T][V]
+    const int *T_e = nullptr;                                 // nullptr: every epoch is T long
+    int normalize = 0;
+    size_t op_bytes = 0;
     cudaStream_t copy = nullptr;                              // read-back stream
     float *K_host = nullptr;
     bool two_buffers = false;                                 // `work` may be split in two blocks: two passes follow the upload
@@ -3151,7 +3184,6 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
     const int S_eps = (E / eps) * eps;
     const bool half16 = half_block(precision, flags);
-    const size_t esz = half16 ? sizeof(__half) : sizeof(float);
     // column-direction pass (E <= 32; fp32 or fp16 block): the column voxels' sums are taken from block A itself, no
     // transposed copy is stored.  FCMA_FLAG_SYM_TRANSPOSED keeps the transposed block B.
     const bool use_cols = sym_uses_cols(precision, E, eps, flags);
@@ -3164,30 +3196,28 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
     if (rows_per_pass < 256)
         return fail(FCMA_ENOMEM, "work buffer too small for the symmetric pipeline: %zu bytes < %zu (256 rows)", work_bytes, 256 * row_bytes);
     const long npass = cdiv(nb, rows_per_pass);
+    // pass p in buffer `buf`: block A = rows [a, a+n) x columns [a, V), and unless the column pass reads A, block B = rows
+    // [a+n, V) x columns [a, a+n) right after it
     struct Pass {
-        long a, n, colsA, t256, nt, rowsB;
+        long a, n, rowsB;
+        CorrBlock A, B;
     };
-    auto geometry = [&](long p) {
+    auto geometry = [&](long p, float *buf) {
         Pass g;
         g.a = start + p * rows_per_pass;
         g.n = nb - p * rows_per_pass < rows_per_pass ? nb - p * rows_per_pass : rows_per_pass;
-        g.colsA = V - g.a, g.t256 = cdiv(g.colsA, 256), g.nt = cdiv(g.n, 256), g.rowsB = V - g.a - g.n;
+        g.rowsB = V - g.a - g.n;
+        g.A = CorrBlock(buf, E, g.n, V - g.a, half16);
+        if (!use_cols) g.B = CorrBlock(g.A.end(), E, g.rowsB, g.n, half16);
         return g;
     };
-    auto blockB = [&](const Pass &g, float *A) {
-        return reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(A) + (size_t)g.nt * g.t256 * E * 65536 * esz);
-    };
-    auto gemm_pass = [&](const Pass &g, float *A, int e_begin, int e_count, bool fixup) -> int {
-        if ((size_t)((g.nt * g.t256 + (use_cols ? 0 : (g.t256 - g.nt) * g.nt)) * E) * 65536 * esz > buf_bytes)
-            return fail(FCMA_ENOMEM, "internal: symmetric pass does not fit the work buffer");
-        SymOut so{use_cols ? nullptr : blockB(g, A)};
-        return launch_corr_mma(op, op, precision, E, T, V, V, g.a, g.n, A, 4, 4, S_eps, st, g.t256, half16 ? 1 : 0, &so,
-                                e_begin, e_count, fixup);
+    auto gemm_pass = [&](const Pass &g, int e_begin, int e_count, bool fixup) -> int {
+        if (g.A.bytes() + g.B.bytes() > buf_bytes) return fail(FCMA_ENOMEM, "internal: symmetric pass does not fit the work buffer");
+        return launch_corr_mma(op, op, precision, T, V, V, g.a, g.A, S_eps, st, &g.B, e_begin, e_count, fixup);
     };
     // normalise + SYRK of one pass: rows of the block, then its columns (or the rows of the transposed copy)
-    auto syrk_pass = [&](const Pass &g, float *A, PassTimer *timer) -> int {
-        int rc = launch_norm_syrk(A, g.n, E, g.colsA, 256, 65536, eps, 1, mask_self ? 0 : -1, 1.0f, K + (size_t)g.a * E * E, 0,
-                                  st, (long)E * 65536, half16 ? 1 : 0);
+    auto syrk_pass = [&](const Pass &g, PassTimer *timer) -> int {
+        int rc = launch_norm_syrk(g.A, eps, 1, mask_self ? 0 : -1, 1.0f, K + (size_t)g.a * E * E, 0, st);
         if (rc) return rc;
         if (timer && (rc = timer->rows_done())) return rc;
         if (hooks && hooks->K_host) {
@@ -3199,13 +3229,8 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
             CUDA_TRY(cudaMemcpyAsync(hooks->K_host + (size_t)g.a * E * E, K + (size_t)g.a * E * E,
                                      (size_t)g.n * E * E * sizeof(float), cudaMemcpyDeviceToHost, hooks->copy));
         }
-        if (g.rowsB > 0 && use_cols)
-            return launch_norm_syrk_cols(A, g.n, E, g.colsA, g.t256, g.n, eps, K + (size_t)g.a * E * E, st, half16 ? 1 : 0,
-                                         (flags & FCMA_FLAG_COLS_TMA) != 0, (flags & FCMA_FLAG_COLS_V2) != 0,
-                                         (flags & FCMA_FLAG_COLS_PAD32) != 0);
-        if (g.rowsB > 0)
-            return launch_norm_syrk(blockB(g, A), g.rowsB, E, g.n, 256, 65536, eps, 1, -1, 1.0f,
-                                    K + (size_t)(g.a + g.n) * E * E, 0, st, (long)E * 65536, half16 ? 1 : 0);
+        if (g.rowsB > 0 && use_cols) return launch_norm_syrk_cols(g.A, g.n, eps, K + (size_t)g.a * E * E, st, flags);
+        if (g.rowsB > 0) return launch_norm_syrk(g.B, eps, 1, -1, 1.0f, K + (size_t)(g.a + g.n) * E * E, 0, st);
         return FCMA_OK;
     };
     float *buf0 = work;
@@ -3215,27 +3240,30 @@ static int run_pipeline_sym(const void *op, int precision, int E, int T, long V,
         // one GEMM launch per uploaded epoch group (a tile needs only its own epoch), the diagonal fix-up after the last
         const long ahead = (two && npass > 1) ? 2 : 1;
         for (int gi = 0; gi < hooks->ngroups; gi++) {
-            int rc = hooks->prepare(hooks->ctx, gi, st);
+            if (hooks->ready && hooks->ready[gi]) CUDA_TRY(cudaStreamWaitEvent(st, hooks->ready[gi], 0));
+            // the grouped entry points pass their own, writable operand buffer as `op`
+            int rc = pack_operand_impl(hooks->epochs, E, T, V, V, hooks->T_e, hooks->normalize, precision, start, V,
+                                       hooks->e0[gi], hooks->cnt[gi], const_cast<void *>(op), hooks->op_bytes, st);
             for (long p = 0; p < ahead && !rc; p++)
-                rc = gemm_pass(geometry(p), p == 0 ? buf0 : buf1, hooks->e0[gi], hooks->cnt[gi], gi == hooks->ngroups - 1);
+                rc = gemm_pass(geometry(p, p == 0 ? buf0 : buf1), hooks->e0[gi], hooks->cnt[gi], gi == hooks->ngroups - 1);
             if (rc) return rc;
         }
         for (long p = 0; p < ahead; p++) {
-            int rc = syrk_pass(geometry(p), p == 0 ? buf0 : buf1, nullptr);
+            int rc = syrk_pass(geometry(p, p == 0 ? buf0 : buf1), nullptr);
             if (rc) return rc;
         }
         first = ahead;
     }
     for (long p = first; p < npass; p++) {
-        const Pass g = geometry(p);
+        const Pass g = geometry(p, buf0);
         PassTimer timer(st);
         int rc = timer.start();
         if (rc) return rc;
-        rc = gemm_pass(g, buf0, 0, E, true);
+        rc = gemm_pass(g, 0, E, true);
         if (rc) return rc;
         rc = timer.gemm_done();
         if (rc) return rc;
-        rc = syrk_pass(g, buf0, &timer);
+        rc = syrk_pass(g, &timer);
         if (rc) return rc;
         rc = timer.end();
         if (rc) return rc;
@@ -3261,7 +3289,6 @@ static int run_classifier_sym(const void *op, int precision, int E, int T, long 
     const bool mask_self = (flags & FCMA_FLAG_MASK_SELF) != 0;
     const int S_eps = (E / eps) * eps;
     const bool half16 = half_block(precision, flags);
-    const size_t esz = half16 ? sizeof(__half) : sizeof(float);
     const size_t row_bytes = fcma_work_bytes_per_row(E, V);
     const long rows_per_pass = (long)(work_bytes / row_bytes) & ~255L;
     if (rows_per_pass < 256) return fail(FCMA_ENOMEM, "work buffer too small for the symmetric pipeline");
@@ -3271,26 +3298,20 @@ static int run_classifier_sym(const void *op, int precision, int E, int T, long 
     double *S = static_cast<double *>(sums.p);
     for (long a = 0; a < V; a += rows_per_pass) {
         const long n = V - a < rows_per_pass ? V - a : rows_per_pass;
-        const long colsA = V - a, t256 = cdiv(colsA, 256), nt = cdiv(n, 256);
-        if ((size_t)(nt * t256 * E) * 65536 * esz > work_bytes) return fail(FCMA_ENOMEM, "internal: symmetric pass does not fit the work buffer");
-        SymOut so{nullptr};
+        const CorrBlock A(work, E, n, V - a, half16), no_B;
+        if (A.bytes() > work_bytes) return fail(FCMA_ENOMEM, "internal: symmetric pass does not fit the work buffer");
         PassTimer timer(st);
         int rc = timer.start();
         if (rc) return rc;
-        rc = launch_corr_mma(op, op, precision, E, T, V, V, a, n, work, 4, 4, S_eps, st, t256, half16 ? 1 : 0, &so);
+        rc = launch_corr_mma(op, op, precision, T, V, V, a, A, S_eps, st, &no_B);
         if (rc) return rc;
         rc = timer.gemm_done();
         if (rc) return rc;
-        const long rb = t256 * (long)E * 65536;                       // elements between the 256-row blocks of the block
-        const long sq = nt * 256 < colsA ? nt * 256 : colsA;          // columns of the diagonal square
-        rc = launch_norm_syrk(work, n, E, sq, 256, 65536, eps, 1, mask_self ? 0 : -1, 1.0f, K, 1, st, (long)E * 65536,
-                              half16 ? 1 : 0, rb, S);
+        const long sq = round_up(n, 256) < A.cols ? round_up(n, 256) : A.cols;   // columns of the diagonal square
+        rc = launch_norm_syrk(A.columns(0, sq), eps, 1, mask_self ? 0 : -1, 1.0f, K, 1, st, S);
         if (rc) return rc;
-        if (colsA > sq) {
-            const float *rest = half16 ? reinterpret_cast<const float *>(reinterpret_cast<const __half *>(work) + (size_t)nt * E * 65536)
-                                       : work + (size_t)nt * E * 65536;
-            rc = launch_norm_syrk(rest, n, E, colsA - sq, 256, 65536, eps, 1, -1, 1.0f, K, 1, st, (long)E * 65536,
-                                  half16 ? 1 : 0, rb, S + (size_t)E * E);
+        if (A.cols > sq) {
+            rc = launch_norm_syrk(A.columns(sq, A.cols), eps, 1, -1, 1.0f, K, 1, st, S + (size_t)E * E);
             if (rc) return rc;
         }
         rc = timer.end();
@@ -3328,24 +3349,6 @@ extern "C" int fcma_voxel_kernels_sym(const void *op, int precision, int E, int 
 // packs each group (voxels [start, V) only) as soon as its event has fired and runs the GEMMs of the first pass -- of the
 // first two passes if `work` holds two blocks -- group by group, so that the upload hides under them; everything else
 // follows as in fcma_voxel_kernels_sym.  Same results.
-struct GroupedCtx {
-    const float *epochs;
-    int E, T;
-    long V, start;
-    const int *T_e;
-    int normalize, precision;
-    void *op;
-    size_t opb;
-    const int *e0, *cnt;
-    void *const *ready;
-};
-static int grouped_prepare(void *vctx, int g, cudaStream_t st)
-{
-    GroupedCtx *c = static_cast<GroupedCtx *>(vctx);
-    if (c->ready && c->ready[g]) CUDA_TRY(cudaStreamWaitEvent(st, (cudaEvent_t)c->ready[g], 0));
-    return pack_operand_impl(c->epochs, c->E, c->T, c->V, c->V, c->T_e, c->normalize, c->precision, c->start, c->V, c->e0[g],
-                             c->cnt[g], c->op, c->opb, st);
-}
 extern "C" int fcma_voxel_kernels_sym_grouped(const float *epochs_dev, const int *T_e, int normalize, void *op_dev,
                                               size_t op_bytes, int precision, int E, int T, long V, long start, long nb,
                                               int eps, int flags, int ngroups, const int *e0, const int *cnt,
@@ -3363,9 +3366,9 @@ extern "C" int fcma_voxel_kernels_sym_grouped(const float *epochs_dev, const int
     }
     if (next != E) return fail(FCMA_EINVAL, "epoch groups must be contiguous and cover [0, E)");
     if (op_bytes < fcma_operand_bytes(precision, E, T, V)) return fail(FCMA_ENOMEM, "packed operand buffer too small");
-    GroupedCtx ctx{epochs_dev, E, T, V, start, T_e, normalize, precision, op_dev, op_bytes, e0, cnt, ready_events};
     SymHostHooks hooks;
-    hooks.ngroups = ngroups, hooks.e0 = e0, hooks.cnt = cnt, hooks.prepare = grouped_prepare, hooks.ctx = &ctx;
+    hooks.ngroups = ngroups, hooks.e0 = e0, hooks.cnt = cnt, hooks.ready = reinterpret_cast<const cudaEvent_t *>(ready_events);
+    hooks.epochs = epochs_dev, hooks.T_e = T_e, hooks.normalize = normalize, hooks.op_bytes = op_bytes;
     hooks.two_buffers = true;
     return run_pipeline_sym(op_dev, precision, E, T, V, start, nb, eps, flags, work_dev, work_bytes, K_dev, (cudaStream_t)stream,
                             &hooks);
@@ -4374,19 +4377,23 @@ __global__ void __launch_bounds__(NG_THREADS, EP == 64 ? 1 : 2)
     }
 }
 
-// (stride_i, ld, chunk_step, t256) address the raw correlation block as launch_norm_syrk's do (tiled: chunk_step = E*65536)
-static int launch_norm_gram_f64(const float *C, long nb, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
-                                int eps, int kind, double gamma, double *K_fit, double *K_pred, cudaStream_t st)
+// over the raw fp32 correlation block C, tiled or strided
+static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
+                                cudaStream_t st)
 {
+    const int E = C.E;
+    const long nb = C.rows;
+    if (C.rc) return C.rc;
     if (E < 1 || E > 64 || eps < 1) return fail(FCMA_EINVAL, "internal: k_norm_gram_f64 needs 1 <= E <= 64, eps >= 1");
-    if (((uintptr_t)C & 15) || (ld & 3) || (stride_i & 3)) return fail(FCMA_EINVAL, "internal: k_norm_gram_f64 needs 16-byte rows");
+    if (((uintptr_t)C.base & 15) || (C.ld & 3) || (C.stride_i & 3)) return fail(FCMA_EINVAL, "internal: k_norm_gram_f64 needs 16-byte rows");
     const long grid = nb < 16L * g_sm_count ? nb : 16L * g_sm_count;
     bool ok = false;
     int rc = FCMA_OK;
     auto go = [&](auto EP, auto KIND) {
         constexpr size_t smem = (size_t)NG_CH * (EP + 4) * sizeof(double) + (size_t)EP * NG_RSP * sizeof(float);
-        rc = launch_kernel(k_norm_gram_f64<EP, KIND>, (unsigned)grid, NG_THREADS, smem, st, "k_norm_gram_f64", C, nb, E, n2,
-                           stride_i, ld, chunk_step, t256, eps, gamma, K_fit, K_pred);
+        rc = launch_kernel(k_norm_gram_f64<EP, KIND>, (unsigned)grid, NG_THREADS, smem, st, "k_norm_gram_f64",
+                           static_cast<const float *>(C.base), nb, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256, eps,
+                           gamma, K_fit, K_pred);
         ok = true;
     };
     auto per_kind = [&](auto EP) {
@@ -4495,25 +4502,6 @@ extern "C" int fcma_host_voxel_kernels(const float *const *raw_host, const float
 // groups and the first pass' GEMM follows group by group; the kernels of a pass are read back while the next pass runs.
 // Device buffers come from the device's default stream-ordered pool, whose release threshold is raised once so that
 // repeated calls reuse the memory instead of going back to the OS.
-struct HostSymCtx {
-    const float *epochs;
-    int E, T;
-    long V;
-    const int *T_e;          // nullptr unless ragged
-    int normalize, precision;
-    void *op;
-    size_t opb;
-    const int *e0, *cnt;
-    cudaEvent_t *landed;     // per group: its epochs are in HBM (recorded on the upload stream)
-};
-static int host_sym_prepare(void *vctx, int g, cudaStream_t st)
-{
-    HostSymCtx *c = static_cast<HostSymCtx *>(vctx);
-    CUDA_TRY(cudaStreamWaitEvent(st, c->landed[g], 0));
-    return pack_operand_impl(c->epochs, c->E, c->T, c->V, c->V, c->T_e, c->normalize, c->precision, 0, c->V, c->e0[g],
-                             c->cnt[g], c->op, c->opb, st);
-}
-
 extern "C" int fcma_host_voxel_kernels_sym(const float *const *raw_host, const int *T_e, int E, long V, int eps,
                                            int precision, int normalize, int flags, int device, long rows_per_pass,
                                            float *K_host)
@@ -4606,9 +4594,9 @@ extern "C" int fcma_host_voxel_kernels_sym(const float *const *raw_host, const i
                                          cudaMemcpyHostToDevice, ss.copy));
             CUDA_TRY(cudaEventRecord(landed.ev[gi], ss.copy));
         }
-        HostSymCtx ctx{(const float *)epochs.p, E, T, V, ragged ? T_e : nullptr, normalize, precision, op.p, opb, e0, cnt, landed.ev};
         SymHostHooks hooks;
-        hooks.ngroups = ng, hooks.e0 = e0, hooks.cnt = cnt, hooks.prepare = host_sym_prepare, hooks.ctx = &ctx;
+        hooks.ngroups = ng, hooks.e0 = e0, hooks.cnt = cnt, hooks.ready = landed.ev;   // recorded on the upload stream
+        hooks.epochs = (const float *)epochs.p, hooks.T_e = ragged ? T_e : nullptr, hooks.normalize = normalize, hooks.op_bytes = opb;
         hooks.copy = ss.copy, hooks.K_host = K_host, hooks.two_buffers = two_blocks;
         rc_run = run_pipeline_sym(op.p, precision, E, T, V, 0, V, eps, flags, (float *)work.p, work_bytes_total, (float *)K.p, st, &hooks);
         // everything enqueued so far must finish before the buffers go back to the pool and the function returns
