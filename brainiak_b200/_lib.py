@@ -73,6 +73,8 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_svm_cv_solve_f64": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double,
                                       c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_svm_cv_solve_wide": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double, c_int,
+                                       c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_searchlight_kernels": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                          c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_voxel_feature_kernels": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_long, c_long, c_long, c_long, c_int,

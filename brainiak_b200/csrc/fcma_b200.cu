@@ -3467,25 +3467,50 @@ __global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E
 // :1126-1162, float Q values, double gradient, eps = tol, TAU = 1e-12; classes grouped with the
 // smaller label first = +1 (svm_group_classes :2246-2326); prediction dec > 0 -> first class
 // :2842-2905), with or without the shrinking heuristic (a template switch of k_svm_cv).  Lane l owns
-// training samples l and l+32 (n_train <= 64).
-struct SvmFold {
+// training samples l + 32 s, s < NS (n_train <= 32 NS; NS is the other template parameter of k_svm_cv).
+// A fold problem of at most N training and N held-out samples: SvmFold (N = 64) for fcma_svm_cv_solve and its
+// neighbours, SvmFoldWide (N = 256) for fcma_svm_cv_solve_wide.
+template <int N>
+struct SvmFoldT {
+    static constexpr int N_MAX = N;
     int n_train, n_pos, n_test, pad;
-    int train_idx[64];        // class (+1) samples first, original order inside a class
-    int test_idx[64];
-    unsigned char test_pos[64];
+    int train_idx[N];         // class (+1) samples first, original order inside a class
+    int test_idx[N];
+    unsigned char test_pos[N];
+};
+using SvmFold = SvmFoldT<64>;
+using SvmFoldWide = SvmFoldT<256>;
+static_assert(sizeof(SvmFold) == 592 && sizeof(SvmFoldWide) == 2320, "the C ABI's fold layouts");
+
+// A warp's staging area in the shrinking solver over N positions: do_shrinking moves the items' state between
+// positions through it
+template <int N>
+struct SvmStageT {
+    static_assert(N <= 256, "map holds positions in one byte");
+    double d[4][N];           // G, G_bar, alpha, QD by position
+    int i[2][N];              // pm, y > 0
+    unsigned char map[N];     // map[new position] = old position
 };
 
-// A warp's staging area in the shrinking solver: do_shrinking moves the items' state between positions through it
-struct SvmStage {
-    double d[4][64];          // G, G_bar, alpha, QD by position
-    int i[2][64];             // pm, y > 0
-    unsigned char map[64];    // map[new position] = old position
+// The shape of a k_svm_cv instantiation with NS slots per lane (N = 32 NS positions).  NS = 2 (fcma_svm_cv_solve and
+// its neighbours): each warp copies Q [64][64] to shared memory and that space stages coef after the solve.  NS = 4, 8
+// (fcma_svm_cv_solve_wide): Q_ab is read from the voxel's [E][E] kernel in global memory -- the problems of a voxel are
+// consecutive, so the warps of a block share one kernel matrix in L1 / L2 -- and a warp's shared memory holds coef [N]
+// doubles.  WORDS = the 64-bit decision words per problem in the entry point's output (1, or 4 for the wide one).
+template <int NS>
+struct SvmShape {
+    static constexpr int N = 32 * NS;
+    static constexpr bool Q_SMEM = NS == 2;
+    using Fold = SvmFoldT<Q_SMEM ? 64 : 256>;
+    static constexpr int WORDS = Fold::N_MAX / 64;
+    static constexpr int WARP_FLOATS = Q_SMEM ? N * N : 2 * N;
+    static_assert(NS % 2 == 0 && N <= Fold::N_MAX, "whole 64-bit words, no wider than the fold");
 };
-// Dynamic shared memory of a k_svm_cv block (4 warps): the warps' Q [64][64] floats, then with shrinking their stages
-constexpr int SVM_Q_FLOATS = 4 * 64 * 64;
+// Dynamic shared memory of a k_svm_cv block (4 warps): the warps' Q or coef, then with shrinking their stages
+template <int NS>
 constexpr size_t svm_smem_bytes(bool shrink)
 {
-    return SVM_Q_FLOATS * sizeof(float) + (shrink ? 4 * sizeof(SvmStage) : 0);
+    return 4 * SvmShape<NS>::WARP_FLOATS * sizeof(float) + (shrink ? 4 * sizeof(SvmStageT<32 * NS>) : 0);
 }
 
 __device__ __forceinline__ void warp_argbest(double &val, int &idx, bool want_max)
@@ -3502,11 +3527,16 @@ __device__ __forceinline__ void warp_argbest(double &val, int &idx, bool want_ma
     }
 }
 
-// The value at position pos of an array held lane-slot-wise (lane l holds positions l and l + 32), on every lane
-template <typename T>
-__device__ __forceinline__ T warp_at(const T (&a)[2], int pos)
+// The value at position pos of an array held lane-slot-wise (lane l holds positions l + 32 s), on every lane.  The slot
+// is picked by a chain of unsigned >= compares: an == compare lets the compiler fold the chain into a[pos >> 5], an
+// indexed array that lives in local memory.
+template <typename T, int NS>
+__device__ __forceinline__ T warp_at(const T (&a)[NS], int pos)
 {
-    return __shfl_sync(0xffffffffu, (pos >> 5) ? a[1] : a[0], pos & 31);
+    T v = a[0];
+#pragma unroll
+    for (int s = 1; s < NS; s++) v = (unsigned)(pos >> 5) >= (unsigned)s ? a[s] : v;
+    return __shfl_sync(0xffffffffu, v, pos & 31);
 }
 
 // libsvm's analytic two-variable step with its clipping order (Solver::Solve, "update alpha[i] and alpha[j]")
@@ -3575,17 +3605,18 @@ __device__ __forceinline__ void smo_pair_update(double &ai, double &aj, double y
     }
 }
 
-// libsvm's calculate_rho over positions [0, cnt) (lane l holds positions l and l + 32): the bounds' min / max in any
+// libsvm's calculate_rho over positions [0, cnt) (lane l holds positions l + 32 s): the bounds' min / max in any
 // order, sum_free added sequentially in position order as libsvm's loop adds it; the same value on every lane
-__device__ __forceinline__ double svm_rho(const double (&y)[2], const double (&G)[2], const double (&alpha)[2], int cnt,
+template <int NS>
+__device__ __forceinline__ double svm_rho(const double (&y)[NS], const double (&G)[NS], const double (&alpha)[NS], int cnt,
                                           double C)
 {
     const int lane = threadIdx.x & 31;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
-    double ub = INF, lb = -INF, yG_free[2];
+    double ub = INF, lb = -INF, yG_free[NS];
     int nr_free = 0;
 #pragma unroll
-    for (int s = 0; s < 2; s++) {
+    for (int s = 0; s < NS; s++) {
         yG_free[s] = 0.0;
         if (lane + 32 * s >= cnt) continue;
         const double yG = y[s] * G[s];
@@ -3613,15 +3644,16 @@ __device__ __forceinline__ double svm_rho(const double (&y)[2], const double (&G
 // The held-out decisions as libsvm's svm_predict_values forms them: dec = sum_k (alpha_k y_k) K(t, k) - rho with the
 // support vectors added sequentially in training order (class +1 first), each product and sum rounded on its own; dec > 0
 // -> the first class.  coef[k] = alpha_k y_k by training index k (per-warp shared memory).  Lane l predicts held-out
-// samples l and l + 32.  bits: bit t set when sample t falls on the first class's side; ok: correctly predicted samples.
-template <typename KT>
-__device__ __forceinline__ void svm_predict(const SvmFold &fd, const KT *__restrict__ Kp, int E, const double *coef,
-                                            double rho, int &ok, unsigned long long &bits)
+// samples l + 32 s.  bits: bit t % 64 of word t / 64 set when sample t falls on the first class's side; ok: correctly
+// predicted samples.
+template <typename KT, int NS, typename Fold>
+__device__ __forceinline__ void svm_predict(const Fold &fd, const KT *__restrict__ Kp, int E, const double *coef,
+                                            double rho, int &ok, unsigned long long (&bits)[NS / 2])
 {
     const int lane = threadIdx.x & 31;
-    bool pos[2], hit[2];
+    bool pos[NS], hit[NS];
 #pragma unroll
-    for (int s = 0; s < 2; s++) {
+    for (int s = 0; s < NS; s++) {
         const int t = lane + 32 * s;
         pos[s] = hit[s] = false;
         if (t >= fd.n_test) continue;
@@ -3634,9 +3666,13 @@ __device__ __forceinline__ void svm_predict(const SvmFold &fd, const KT *__restr
         pos[s] = __dsub_rn(sum, rho) > 0;
         hit[s] = pos[s] == (fd.test_pos[t] != 0);
     }
-    bits = (unsigned long long)__ballot_sync(0xffffffffu, pos[0]) |
-           ((unsigned long long)__ballot_sync(0xffffffffu, pos[1]) << 32);
-    ok = __popc(__ballot_sync(0xffffffffu, hit[0])) + __popc(__ballot_sync(0xffffffffu, hit[1]));
+#pragma unroll
+    for (int w = 0; w < NS / 2; w++)
+        bits[w] = (unsigned long long)__ballot_sync(0xffffffffu, pos[2 * w]) |
+                  ((unsigned long long)__ballot_sync(0xffffffffu, pos[2 * w + 1]) << 32);
+    ok = 0;
+#pragma unroll
+    for (int s = 0; s < NS; s++) ok += __popc(__ballot_sync(0xffffffffu, hit[s]));
 }
 
 // Kernel element type KT: float (the FCMA kernels) or double (searchlight kernels).  Either way Q is float and QD, the
@@ -3647,35 +3683,40 @@ __device__ __forceinline__ void svm_predict(const SvmFold &fd, const KT *__restr
 //
 // SHRINK adds libsvm's shrinking heuristic (scikit-learn's default shrinking=True): Solver::do_shrinking, be_shrunk,
 // reconstruct_gradient, swap_index and the counter / unshrink logic of Solver::Solve restated for one warp.  Lanes own
-// POSITIONS lane and lane+32 of libsvm's permuted arrays; an item's state (y, alpha, G, G_bar, QD and its index `pm` in
+// POSITIONS lane + 32 s of libsvm's permuted arrays; an item's state (y, alpha, G, G_bar, QD and its index `pm` in
 // the unpermuted sub-problem = active_set[]) travels between positions through the warp's SvmStage when do_shrinking
 // swaps; Q stays in the unpermuted order and is addressed through pm.  Working-set selection, the G update and rho run
 // over [0, active); G_bar over all n.  Without SHRINK, active = n and every item stays at its own position.
-template <typename KT, bool SHRINK>
+//
+// NS = slots per lane (SvmShape): every per-position step is a loop over the NS slots of a lane, scanned in ascending
+// position with the same ">=" / "<=" tie rules, so the later index still wins.
+template <typename KT, bool SHRINK, int NS>
 __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long nv, int E, int nfolds,
-                                               const SvmFold *__restrict__ folds, double C, double eps, int max_iter,
-                                               int *__restrict__ correct, int *__restrict__ iters,
-                                               unsigned long long *__restrict__ dec_bits, const KT *__restrict__ Kpred)
+                                               const typename SvmShape<NS>::Fold *__restrict__ folds, double C,
+                                               double eps, int max_iter, int *__restrict__ correct,
+                                               int *__restrict__ iters, unsigned long long *__restrict__ dec_bits,
+                                               const KT *__restrict__ Kpred)
 {
-    extern __shared__ float s_q[];   // svm_smem_bytes(SHRINK): [4 warps][64][64] Q, then with SHRINK [4 warps] SvmStage
+    using SH = SvmShape<NS>;
+    extern __shared__ float s_q[];   // svm_smem_bytes<NS>(SHRINK): [4 warps] Q or coef, then with SHRINK [4 warps] stages
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long prob = (long)blockIdx.x * 4 + warp;
     if (prob >= nv * nfolds) return;
     const long v = prob / nfolds;
     const int f = (int)(prob - v * nfolds);
-    const SvmFold &fd = folds[f];
+    const typename SH::Fold &fd = folds[f];
     const int n = fd.n_train;
     const KT *Kv = K + (size_t)v * E * E;
     const KT *Kp = sizeof(KT) == 4 ? Kv : Kpred + (size_t)v * E * E;
-    float *Q = s_q + (size_t)warp * 64 * 64;
+    float *Q = s_q + (size_t)warp * SH::WARP_FLOATS;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
     const double TAU = 1e-12;
     const unsigned FULL = 0xffffffffu;
 
     // the item at a position: its index in the unpermuted sub-problem (Q's row / column) and its y, on every lane; and
     // the index of this lane's slot s.  Without shrinking that is the position itself and y follows from it.
-    int pm[2];
-    double y[2];
+    int pm[NS];
+    double y[NS];
     auto index_at = [&](int pos) {
         if constexpr (SHRINK) return warp_at(pm, pos); else return pos;
     };
@@ -3686,11 +3727,11 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         if constexpr (SHRINK) return warp_at(y, pos); else return pos < fd.n_pos ? 1.0 : -1.0;
     };
 
-    // sub-problem in libsvm's order; Q_ab = (float)(y_a y_b K_ab)
-    int idx[2];
-    double alpha[2], G[2], Gb[2], QD[2];
+    // sub-problem in libsvm's order; Q_ab = (float)(y_a y_b K_ab).  idx: the kernel row / column of this lane's items
+    int idx[NS];
+    double alpha[NS], G[NS], Gb[NS], QD[NS];
 #pragma unroll
-    for (int s = 0; s < 2; s++) {
+    for (int s = 0; s < NS; s++) {
         const int k = lane + 32 * s;
         pm[s] = k < n ? k : 0;
         idx[s] = k < n ? fd.train_idx[k] : 0;
@@ -3699,18 +3740,40 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         G[s] = -1.0;   // p = -1
         Gb[s] = 0.0;
     }
-    for (int a = 0; a < n; a++) {
-        const int ia = fd.train_idx[a];
-        const float ya = a < fd.n_pos ? 1.f : -1.f;
+    if constexpr (SH::Q_SMEM) {
+        for (int a = 0; a < n; a++) {
+            const int ia = fd.train_idx[a];
+            const float ya = a < fd.n_pos ? 1.f : -1.f;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
-            const int k = lane + 32 * s;
-            if (k < n) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + idx[s]];
+            for (int s = 0; s < NS; s++) {
+                const int k = lane + 32 * s;
+                if (k < n) Q[a * 64 + k] = ya * (float)y[s] * (float)Kv[(size_t)ia * E + idx[s]];
+            }
         }
+        __syncwarp();
     }
-    __syncwarp();
 #pragma unroll
-    for (int s = 0; s < 2; s++) QD[s] = lane + 32 * s < n ? (double)Kv[(size_t)idx[s] * E + idx[s]] : 0.0;
+    for (int s = 0; s < NS; s++) QD[s] = lane + 32 * s < n ? (double)Kv[(size_t)idx[s] * E + idx[s]] : 0.0;
+
+    // row a of Q (a an unpermuted index): Q_ab for the item of this lane's slot s (q_own) or for any unpermuted b (q_at),
+    // from the warp's copy or straight from the kernel
+    struct QRow {
+        const float *q;
+        const KT *k;
+        float y;
+    };
+    auto q_row = [&](int a) {
+        if constexpr (SH::Q_SMEM) return QRow{Q + a * 64, nullptr, 0.f};
+        else return QRow{nullptr, Kv + (size_t)fd.train_idx[a] * E, a < fd.n_pos ? 1.f : -1.f};
+    };
+    auto q_own = [&](const QRow &r, int s) -> float {
+        if constexpr (SH::Q_SMEM) return r.q[own_index(s)];
+        else return r.y * (float)y[s] * (float)r.k[idx[s]];
+    };
+    auto q_at = [&](const QRow &r, int b) -> float {
+        if constexpr (SH::Q_SMEM) return r.q[b];
+        else return r.y * (b < fd.n_pos ? 1.f : -1.f) * (float)r.k[fd.train_idx[b]];
+    };
 
     int active = n;
     bool unshrink = false;
@@ -3721,7 +3784,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         double Gmax = -INF;
         i = -1;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= active) continue;
             double cand = -INF;
@@ -3739,13 +3802,13 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         j = -1;
         if (i < 0) return true;
         const double yi = y_at(i), QDi = warp_at(QD, i);
-        const float *Qi = Q + index_at(i) * 64;
+        const QRow Qi = q_row(index_at(i));
         double Gmax2 = -INF, obj_min = INF;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= active) continue;
-            const double Qik = (double)Qi[own_index(s)];
+            const double Qik = (double)q_own(Qi, s);
             if (y[s] > 0) {
                 if (!(alpha[s] <= 0)) {
                     const double gd = Gmax + G[s];
@@ -3789,7 +3852,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         if (active == n) return;
         int nr_free = 0;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= active && k < n) G[s] = __dadd_rn(Gb[s], -1.0);
             if (k < active && !(alpha[s] >= C) && !(alpha[s] <= 0)) ++nr_free;
@@ -3802,10 +3865,10 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
             const int pm_j = warp_at(pm, jj);
             if (a_j >= C || a_j <= 0) continue;
 #pragma unroll
-            for (int s = 0; s < 2; s++) {
+            for (int s = 0; s < NS; s++) {
                 const int k = lane + 32 * s;
                 if (k >= active && k < n) {
-                    const float q = by_rows ? Q[pm[s] * 64 + pm_j] : Q[pm_j * 64 + pm[s]];
+                    const float q = by_rows ? q_at(q_row(pm[s]), pm_j) : q_at(q_row(pm_j), pm[s]);
                     G[s] = __dadd_rn(G[s], __dmul_rn(a_j, (double)q));
                 }
             }
@@ -3816,7 +3879,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
     auto do_shrinking = [&]() {
         double g1 = -INF, g2 = -INF;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= active) continue;
             const bool up = alpha[s] >= C, low = alpha[s] <= 0;
@@ -3839,9 +3902,10 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
             reconstruct();
             active = n;
         }
-        bool fl[2];
+        // the be-shrunk mask: bit p % 64 of word p / 64 for position p
+        bool fl[NS];
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             fl[s] = false;
             if (k >= active) continue;
@@ -3850,26 +3914,42 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
             else if (alpha[s] <= 0)
                 fl[s] = y[s] > 0 ? (G[s] > g2) : (G[s] > g1);
         }
-        unsigned long long F = (unsigned long long)__ballot_sync(FULL, fl[0]) |
-                               ((unsigned long long)__ballot_sync(FULL, fl[1]) << 32);
-        if (F == 0ull) return;
-        SvmStage &stg = reinterpret_cast<SvmStage *>(s_q + SVM_Q_FLOATS)[warp];
-        stg.map[lane] = (unsigned char)lane;
-        stg.map[lane + 32] = (unsigned char)(lane + 32);
+        unsigned long long F[NS / 2], any = 0ull;
+#pragma unroll
+        for (int w = 0; w < NS / 2; w++) {
+            F[w] = (unsigned long long)__ballot_sync(FULL, fl[2 * w]) |
+                   ((unsigned long long)__ballot_sync(FULL, fl[2 * w + 1]) << 32);
+            any |= F[w];
+        }
+        if (any == 0ull) return;
+        auto flagged = [&](int p) {   // the word picked as warp_at picks a slot
+            const unsigned word = (unsigned)(p >> 6);
+            unsigned long long w = F[0];
+            int bit = p;
+#pragma unroll
+            for (int k = 1; k < NS / 2; k++)
+                if (word >= (unsigned)k) {
+                    w = F[k];
+                    bit = p - 64 * k;
+                }
+            return ((w >> bit) & 1ull) != 0;
+        };
+        SvmStageT<SH::N> &stg = reinterpret_cast<SvmStageT<SH::N> *>(s_q + 4 * SH::WARP_FLOATS)[warp];
+#pragma unroll
+        for (int s = 0; s < NS; s++) stg.map[lane + 32 * s] = (unsigned char)(lane + 32 * s);
         __syncwarp();
         int act = active, swaps = 0;
         if (lane == 0) {
             // the serial scan of libsvm (flags travel with the items: after swap_index(i, act) position i holds the
-            // unflagged item and position act the flagged one)
+            // unflagged item and position act the flagged one; the scan reads neither position again)
             for (int i = 0; i < act; i++)
-                if ((F >> i) & 1ull) {
+                if (flagged(i)) {
                     act--;
                     while (act > i) {
-                        if (!((F >> act) & 1ull)) {
+                        if (!flagged(act)) {
                             const unsigned char t = stg.map[i];
                             stg.map[i] = stg.map[act];
                             stg.map[act] = t;
-                            F ^= (1ull << i) | (1ull << act);
                             ++swaps;
                             break;
                         }
@@ -3882,7 +3962,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         active = act;
         if (swaps == 0) return;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             stg.d[0][k] = G[s];
             stg.d[1][k] = Gb[s];
@@ -3893,7 +3973,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         }
         __syncwarp();
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= n) continue;
             const int src = stg.map[k];
@@ -3903,6 +3983,7 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
             QD[s] = stg.d[3][src];
             pm[s] = stg.i[0][src];
             y[s] = stg.i[1][src] ? 1.0 : -1.0;
+            if constexpr (!SH::Q_SMEM) idx[s] = fd.train_idx[pm[s]];
         }
         __syncwarp();
     };
@@ -3931,17 +4012,17 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
         const double yi = y_at(i), yj = y_at(j), QDi = warp_at(QD, i), QDj = warp_at(QD, j);
         const double Gi = warp_at(G, i), Gj = warp_at(G, j);
         const int pmi = index_at(i), pmj = index_at(j);
-        const float *Qi = Q + pmi * 64, *Qj = Q + pmj * 64;
+        const QRow Qi = q_row(pmi), Qj = q_row(pmj);
         double ai = warp_at(alpha, i), aj = warp_at(alpha, j);
         const double old_ai = ai, old_aj = aj;
-        smo_pair_update(ai, aj, yi, yj, QDi, QDj, (double)Qi[pmj], Gi, Gj, C);
+        smo_pair_update(ai, aj, yi, yj, QDi, QDj, (double)q_at(Qi, pmj), Gi, Gj, C);
         const double dai = ai - old_ai, daj = aj - old_aj;
         const bool ui = old_ai >= C, uj = old_aj >= C, ui2 = ai >= C, uj2 = aj >= C;   // G_bar's bound changes
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
+        for (int s = 0; s < NS; s++) {
             const int k = lane + 32 * s;
             if (k >= n) continue;
-            const double qi = (double)Qi[own_index(s)], qj = (double)Qj[own_index(s)];
+            const double qi = (double)q_own(Qi, s), qj = (double)q_own(Qj, s);
             // G[k] += Q_i[k]*dai + Q_j[k]*daj, no FMA contraction (as the reference compiles it)
             if (k < active) G[s] = __dadd_rn(G[s], __dadd_rn(__dmul_rn(qi, dai), __dmul_rn(qj, daj)));
             if constexpr (SHRINK) {
@@ -3956,21 +4037,24 @@ __global__ void __launch_bounds__(128) k_svm_cv(const KT *__restrict__ K, long n
     // ---- rho (calculate_rho over the active positions: all of them unless max_iter cut the loop)
     const double rho = svm_rho(y, G, alpha, active, C);
 
-    // ---- predict the held-out samples in training order: Q is no longer read, its space stages alpha_k y_k by
-    // unpermuted index
+    // ---- predict the held-out samples in training order: the warp's shared memory (Q, no longer read, or the coef
+    // space) stages alpha_k y_k by unpermuted index
     double *coef = reinterpret_cast<double *>(Q);
     __syncwarp();
 #pragma unroll
-    for (int s = 0; s < 2; s++)
+    for (int s = 0; s < NS; s++)
         if (lane + 32 * s < n) coef[own_index(s)] = alpha[s] * y[s];
     __syncwarp();
     int ok;
-    unsigned long long bits;
-    svm_predict(fd, Kp, E, coef, rho, ok, bits);
+    unsigned long long bits[NS / 2];
+    svm_predict<KT, NS>(fd, Kp, E, coef, rho, ok, bits);
     if (lane == 0) {
         if (correct) correct[prob] = ok;
         if (iters) iters[prob] = iter;
-        if (dec_bits) dec_bits[prob] = bits;
+        if (dec_bits) {
+#pragma unroll
+            for (int w = 0; w < SH::WORDS; w++) dec_bits[prob * SH::WORDS + w] = w < NS / 2 ? bits[w] : 0ull;
+        }
     }
 }
 
@@ -3984,17 +4068,17 @@ extern "C" int fcma_shrink_kernels(float *K_dev, long nv, int E, int *digits_dev
     return FCMA_OK;
 }
 
-template <typename KT>
-static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds, const void *folds_host, double C,
-                       double tol, int max_iter, int shrinking, int *correct_dev, int *iters_dev,
-                       unsigned long long *bits_dev, void *stream);
+template <typename KT, typename Fold>
+static int svm_cv_impl(const char *who, const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds,
+                       const void *folds_host, double C, double tol, int max_iter, int shrinking, int *correct_dev,
+                       int *iters_dev, unsigned long long *bits_dev, void *stream);
 extern "C" int fcma_svm_cv_precomputed(const float *K_dev, long nv, int E, int nfolds, const void *folds_host,
                                        double C, double tol, int max_iter, int *correct_dev, int *iters_dev,
                                        void *stream)
 {
     if (!correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_precomputed: null output");
-    return svm_cv_impl<float>(K_dev, nullptr, nv, E, nfolds, folds_host, C, tol, max_iter, 0, correct_dev, iters_dev,
-                              nullptr, stream);
+    return svm_cv_impl<float, SvmFold>("fcma_svm_cv_precomputed", K_dev, nullptr, nv, E, nfolds, folds_host, C, tol,
+                                       max_iter, 0, correct_dev, iters_dev, nullptr, stream);
 }
 // the general form: `shrinking` selects the restatement of libsvm's shrinking heuristic (scikit-learn's default); bits_dev
 // (optional) receives the binary DECISION of every held-out sample (bit t of bits_dev[v * nproblems + p]) -- the building
@@ -4004,8 +4088,8 @@ extern "C" int fcma_svm_cv_solve(const float *K_dev, long nv, int E, int nproble
                                  unsigned long long *bits_dev, int *iters_dev, void *stream)
 {
     if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve: no output requested");
-    return svm_cv_impl<float>(K_dev, nullptr, nv, E, nproblems, folds_host, C, tol, max_iter, shrinking, correct_dev,
-                              iters_dev, bits_dev, stream);
+    return svm_cv_impl<float, SvmFold>("fcma_svm_cv_precomputed", K_dev, nullptr, nv, E, nproblems, folds_host, C, tol,
+                                       max_iter, shrinking, correct_dev, iters_dev, bits_dev, stream);
 }
 // the same solver on fp64 kernels: Q_ab = (float)(y_a y_b K_fit_ab), QD_a = K_fit_aa and the decisions
 // sum_k alpha_k y_k K_pred[t][k] - rho in double.  K_pred may be K_fit (linear kernel).
@@ -4015,37 +4099,60 @@ extern "C" int fcma_svm_cv_solve_f64(const double *K_fit_dev, const double *K_pr
 {
     if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64: no output requested");
     if (!K_pred_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64: null K_pred");
-    return svm_cv_impl<double>(K_fit_dev, K_pred_dev, nv, E, nproblems, folds_host, C, tol, max_iter, shrinking,
-                               correct_dev, iters_dev, bits_dev, stream);
+    return svm_cv_impl<double, SvmFold>("fcma_svm_cv_precomputed", K_fit_dev, K_pred_dev, nv, E, nproblems, folds_host, C,
+                                        tol, max_iter, shrinking, correct_dev, iters_dev, bits_dev, stream);
 }
-template <typename KT>
-static int svm_cv_impl(const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds, const void *folds_host, double C,
-                       double tol, int max_iter, int shrinking, int *correct_dev, int *iters_dev,
-                       unsigned long long *bits_dev, void *stream)
+// fcma_svm_cv_solve for up to 256 epochs: SvmFoldWide problems, 4 decision words per problem.  k_svm_cv runs with 4
+// slots per lane when no problem has more than 128 training or held-out samples, else with 8.
+extern "C" int fcma_svm_cv_solve_wide(const float *K_dev, long nv, int E, int nproblems, const void *folds_host,
+                                      double C, double tol, int max_iter, int shrinking, int *correct_dev,
+                                      unsigned long long *bits_dev, int *iters_dev, void *stream)
 {
+    if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_wide: no output requested");
+    return svm_cv_impl<float, SvmFoldWide>("fcma_svm_cv_solve_wide", K_dev, nullptr, nv, E, nproblems, folds_host, C,
+                                           tol, max_iter, shrinking, correct_dev, iters_dev, bits_dev, stream);
+}
+// Checks the fold problems (who: the entry point the messages name) and launches k_svm_cv on them: SvmFold problems
+// with NS = 2, SvmFoldWide problems with the fewest slots per lane that hold every problem
+template <typename KT, typename Fold>
+static int svm_cv_impl(const char *who, const KT *K_dev, const KT *Kpred_dev, long nv, int E, int nfolds,
+                       const void *folds_host, double C, double tol, int max_iter, int shrinking, int *correct_dev,
+                       int *iters_dev, unsigned long long *bits_dev, void *stream)
+{
+    constexpr int NMAX = Fold::N_MAX;
     int rc = check_device();
     if (rc) return rc;
-    if (!K_dev || !folds_host || nv <= 0 || E <= 0 || E > 64 || nfolds <= 0 || nfolds > 4096)
-        return fail(FCMA_EINVAL, "fcma_svm_cv_precomputed: bad arguments (E <= 64, at most 4096 fold problems)");
-    if (!(C > 0) || !(tol > 0)) return fail(FCMA_EINVAL, "fcma_svm_cv_precomputed: C and tol must be positive");
-    const SvmFold *fh = reinterpret_cast<const SvmFold *>(folds_host);
+    if (!K_dev || !folds_host || nv <= 0 || E <= 0 || E > NMAX || nfolds <= 0 || nfolds > 4096)
+        return fail(FCMA_EINVAL, "%s: bad arguments (E <= %d, at most 4096 fold problems)", who, NMAX);
+    if (!(C > 0) || !(tol > 0)) return fail(FCMA_EINVAL, "%s: C and tol must be positive", who);
+    const Fold *fh = reinterpret_cast<const Fold *>(folds_host);
+    int widest = 0;
     for (int f = 0; f < nfolds; f++) {
-        if (fh[f].n_train < 2 || fh[f].n_train > 64 || fh[f].n_test < 0 || fh[f].n_test > 64 || fh[f].n_pos < 1 ||
+        if (fh[f].n_train < 2 || fh[f].n_train > NMAX || fh[f].n_test < 0 || fh[f].n_test > NMAX || fh[f].n_pos < 1 ||
             fh[f].n_pos >= fh[f].n_train)
-            return fail(FCMA_EINVAL, "fold %d: need both classes in the training part and <= 64 samples", f);
+            return fail(FCMA_EINVAL, "fold %d: need both classes in the training part and <= %d samples", f, NMAX);
         for (int k = 0; k < fh[f].n_train; k++)
             if (fh[f].train_idx[k] < 0 || fh[f].train_idx[k] >= E) return fail(FCMA_EINVAL, "fold %d: bad train index", f);
         for (int k = 0; k < fh[f].n_test; k++)
             if (fh[f].test_idx[k] < 0 || fh[f].test_idx[k] >= E) return fail(FCMA_EINVAL, "fold %d: bad test index", f);
+        widest = std::max(widest, std::max(fh[f].n_train, fh[f].n_test));
     }
     cudaStream_t st = (cudaStream_t)stream;
     AsyncBuf fd_buf;
-    CUDA_TRY(fd_buf.alloc(sizeof(SvmFold) * nfolds, st));
-    SvmFold *fd = static_cast<SvmFold *>(fd_buf.p);
-    CUDA_TRY(cudaMemcpyAsync(fd, fh, sizeof(SvmFold) * nfolds, cudaMemcpyHostToDevice, st));
-    return launch_kernel(shrinking ? k_svm_cv<KT, true> : k_svm_cv<KT, false>, (unsigned)cdiv(nv * nfolds, 4), 128,
-                         svm_smem_bytes(shrinking), st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C, tol, max_iter,
-                         correct_dev, iters_dev, bits_dev, Kpred_dev);
+    CUDA_TRY(fd_buf.alloc(sizeof(Fold) * nfolds, st));
+    Fold *fd = static_cast<Fold *>(fd_buf.p);
+    CUDA_TRY(cudaMemcpyAsync(fd, fh, sizeof(Fold) * nfolds, cudaMemcpyHostToDevice, st));
+    auto go = [&](auto ns) {
+        constexpr int NS = decltype(ns)::value;
+        static_assert(std::is_same<typename SvmShape<NS>::Fold, Fold>::value, "fold layout of the instantiation");
+        return launch_kernel(shrinking ? k_svm_cv<KT, true, NS> : k_svm_cv<KT, false, NS>, (unsigned)cdiv(nv * nfolds, 4),
+                             128, svm_smem_bytes<NS>(shrinking), st, "k_svm_cv", K_dev, nv, E, nfolds, fd, C, tol,
+                             max_iter, correct_dev, iters_dev, bits_dev, Kpred_dev);
+    };
+    if constexpr (NMAX == 64)
+        return go(IntC<2>{});
+    else
+        return widest <= 128 ? go(IntC<4>{}) : go(IntC<8>{});
 }
 
 // ============================================================================================

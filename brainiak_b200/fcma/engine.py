@@ -580,6 +580,16 @@ class _SvmFold(ctypes.Structure):
                 ("test_pos", ctypes.c_ubyte * 64)]
 
 
+class _SvmFoldWide(ctypes.Structure):
+    """The fold problem of fcma_svm_cv_solve_wide: _SvmFold with room for 256 training and 256 held-out samples."""
+    _fields_ = [("n_train", ctypes.c_int), ("n_pos", ctypes.c_int), ("n_test", ctypes.c_int),
+                ("pad", ctypes.c_int), ("train_idx", ctypes.c_int * 256), ("test_idx", ctypes.c_int * 256),
+                ("test_pos", ctypes.c_ubyte * 256)]
+
+
+SVM_WIDE_MAX_EPOCHS = 256
+
+
 def shrink_kernels_(K, return_digits=False):
     """In-place decimal shrink (voxelselector.py:409-412) of ``K`` = float32 CUDA ``[nv, E, E]``."""
     lib = _lib.load()
@@ -591,9 +601,10 @@ def shrink_kernels_(K, return_digits=False):
     return digits
 
 
-def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True):
+def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True, max_epochs=64):
     """True if ``cross_val_score(clf, K, labels, cv=StratifiedKFold(num_folds))`` can run on the GPU:
-    ``SVC(kernel='precomputed')`` without class weights / probability / tie breaking, E <= 64; two classes, or more
+    ``SVC(kernel='precomputed')`` without class weights / probability / tie breaking, E <= ``max_epochs`` (64, or up to
+    ``SVM_WIDE_MAX_EPOCHS``, which ``svm_cv_precomputed`` solves with the wide solver above 64); two classes, or more
     (one-vs-one, as libsvm does) when every class is in the training part of every fold.
 
     The GPU solver restates libsvm's SMO with and without the shrinking heuristic (``clf.shrinking``; the reference's tests
@@ -605,7 +616,8 @@ def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True):
     if getattr(clf, 'shrinking', False) and not allow_shrinking:
         return False
     # scikit-learn >= 1.9 uses the string 'deprecated' as the default of `probability`
-    if clf.class_weight is not None or getattr(clf, 'probability', False) is True or E > 64 or num_folds > 64:
+    if clf.class_weight is not None or getattr(clf, 'probability', False) is True or E > min(max_epochs, SVM_WIDE_MAX_EPOCHS) \
+            or num_folds > 64:
         return False
     y = np.asarray(labels)
     classes = np.unique(y)
@@ -614,7 +626,7 @@ def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True):
     if len(classes) < 2 or getattr(clf, 'break_ties', False):
         return False
     try:
-        make_svm_folds(y, num_folds)
+        svm_folds_for(y, num_folds, E)
     except ValueError:
         return False
     return True
@@ -657,6 +669,7 @@ class SvmFolds:
         self.structs, self.n_test, self.classes, self.pairs, self.test_labels = structs, n_test, classes, pairs, test_labels
         self.num_folds = len(n_test)
         self.nproblems = len(structs)
+        self.wide = structs._type_ is _SvmFoldWide     # for fcma_svm_cv_solve_wide
 
     def __iter__(self):          # (structs, n_test) unpacking of the two-class form
         return iter((self.structs, self.n_test))
@@ -667,6 +680,22 @@ def make_svm_folds(labels, num_folds):
     (StratifiedKFold(n_splits, shuffle=False), reference voxelselector.py:44-45).  With k > 2 classes each fold becomes
     k(k-1)/2 two-class problems (libsvm's one-vs-one: the pair (a, b), a < b, trains on the fold's samples of those two
     classes with class a as +1 and is evaluated on ALL held-out samples of the fold)."""
+    return _build_svm_folds(labels, num_folds, _SvmFold, 64)
+
+
+def make_svm_folds_wide(labels, num_folds):
+    """``make_svm_folds`` for fcma_svm_cv_solve_wide: the same splits and problems, up to 256 training and 256 held-out
+    samples per problem."""
+    return _build_svm_folds(labels, num_folds, _SvmFoldWide, 256)
+
+
+def svm_folds_for(labels, num_folds, E):
+    """The fold problems ``svm_cv_precomputed`` solves E-epoch kernels with: ``make_svm_folds`` up to 64 epochs, else
+    ``make_svm_folds_wide``."""
+    return make_svm_folds(labels, num_folds) if E <= 64 else make_svm_folds_wide(labels, num_folds)
+
+
+def _build_svm_folds(labels, num_folds, struct, limit):
     from sklearn import model_selection
     y = np.asarray(labels)
     classes = np.unique(y)
@@ -676,19 +705,19 @@ def make_svm_folds(labels, num_folds):
     k = len(classes)
     pairs = [(a, b) for a in range(k) for b in range(a + 1, k)]
     skf = model_selection.StratifiedKFold(n_splits=num_folds, shuffle=False)
-    folds = (_SvmFold * (num_folds * len(pairs)))()
+    folds = (struct * (num_folds * len(pairs)))()
     n_test, test_labels = [], []
     for f, (tr, te) in enumerate(skf.split(np.zeros((len(y), 1)), y)):
-        if len(te) > 64:
-            raise ValueError("more than 64 held-out samples in a fold")
+        if len(te) > limit:
+            raise ValueError("more than %d held-out samples in a fold" % limit)
         for q, (a, b) in enumerate(pairs):
             pos = [int(i) for i in tr if code[i] == a]     # smaller label first = class +1
             neg = [int(i) for i in tr if code[i] == b]
             if not pos or not neg:
                 raise ValueError("a training fold misses a class")
             order = pos + neg
-            if len(order) > 64:
-                raise ValueError("more than 64 training samples in a class pair")
+            if len(order) > limit:
+                raise ValueError("more than %d training samples in a class pair" % limit)
             fd = folds[f * len(pairs) + q]
             fd.n_train, fd.n_pos, fd.n_test = len(order), len(pos), len(te)
             for j, i in enumerate(order):
@@ -702,18 +731,21 @@ def make_svm_folds(labels, num_folds):
 
 
 def _ovo_vote(bits, folds):
-    """libsvm's svm_predict vote on the device: ``bits`` int64 ``[nv, nproblems]`` (bit t = held-out sample t on the side
-    of the pair's first class) -> number of correctly predicted held-out samples per (voxel, fold).  Ties go to the
-    smallest class index (the first maximum), as in libsvm."""
+    """libsvm's svm_predict vote on the device: ``bits`` int64 ``[nv, nproblems]``, or ``[nv, nproblems, words]`` (bit
+    t % 64 of word t // 64 = held-out sample t on the side of the pair's first class) -> number of correctly predicted
+    held-out samples per (voxel, fold).  Ties go to the smallest class index (the first maximum), as in libsvm."""
+    if bits.dim() == 2:
+        bits = bits[:, :, None]
     nv = bits.shape[0]
     k, npairs = len(folds.classes), len(folds.pairs)
     correct = torch.zeros((nv, folds.num_folds), dtype=torch.int32, device=bits.device)
     for f in range(folds.num_folds):
         nt = int(folds.n_test[f])
-        shifts = torch.arange(nt, device=bits.device, dtype=torch.int64)
+        t = torch.arange(nt, device=bits.device, dtype=torch.int64)
+        word, shifts = t // 64, t % 64
         votes = torch.zeros((nv, nt, k), dtype=torch.int32, device=bits.device)
         for q, (a, b) in enumerate(folds.pairs):
-            side = ((bits[:, f * npairs + q, None] >> shifts[None, :]) & 1).to(torch.int32)   # [nv, nt]
+            side = ((bits[:, f * npairs + q, word] >> shifts[None, :]) & 1).to(torch.int32)   # [nv, nt]
             votes[:, :, a] += side
             votes[:, :, b] += 1 - side
         # first maximum: argmax of votes * k + (k - 1 - class)
@@ -742,7 +774,8 @@ def _svm_cv(solve, kernels, K, labels, num_folds, C, tol, max_iter, shrinking, f
     with torch.cuda.device(K.device):
         iters = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if return_iters else None
         correct = torch.empty((nv, nprob), dtype=torch.int32, device=K.device) if two else None
-        bits = None if two else torch.empty((nv, nprob), dtype=torch.int64, device=K.device)
+        bits = None if two else torch.empty((nv, nprob, 4) if folds.wide else (nv, nprob), dtype=torch.int64,
+                                            device=K.device)
         _lib.check(solve(*kernels, nv, E, nprob, ctypes.cast(folds.structs, ctypes.c_void_p), float(C), float(tol),
                          _max_iter_arg(max_iter), 1 if shrinking else 0, _ptr(correct) if two else None,
                          _ptr(bits) if not two else None, _ptr(iters) if iters is not None else None, _stream_ptr()))
@@ -758,9 +791,18 @@ def svm_cv_precomputed(K, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, folds
     """Mean cross-validation accuracy of ``SVC(kernel='precomputed', C, tol, shrinking)`` for every kernel of
     ``K`` (float32 CUDA ``[nv, E, E]``), computed by the batched GPU SMO solver.  Equivalent to
     ``cross_val_score(clf, K[v], y=labels, cv=StratifiedKFold(num_folds)).mean()`` per voxel; more than two classes are
-    handled one-vs-one with libsvm's vote; ``shrinking`` selects the restatement of libsvm's shrinking heuristic."""
-    return _svm_cv(_lib.load().fcma_svm_cv_solve, (_ptr(K),), K, labels, num_folds, C, tol, max_iter, shrinking, folds,
-                   return_iters)
+    handled one-vs-one with libsvm's vote; ``shrinking`` selects the restatement of libsvm's shrinking heuristic.
+    E <= 64 runs fcma_svm_cv_solve on ``make_svm_folds`` problems, 64 < E <= 256 fcma_svm_cv_solve_wide on
+    ``make_svm_folds_wide`` problems (``folds``, when given, must be of that form)."""
+    lib = _lib.load()
+    E = K.shape[1]
+    wide = E > 64
+    if folds is None:
+        folds = svm_folds_for(labels, num_folds, E)
+    elif folds.wide != wide:
+        raise ValueError("%d epochs need %s folds" % (E, "make_svm_folds_wide" if wide else "make_svm_folds"))
+    solve = lib.fcma_svm_cv_solve_wide if wide else lib.fcma_svm_cv_solve
+    return _svm_cv(solve, (_ptr(K),), K, labels, num_folds, C, tol, max_iter, shrinking, folds, return_iters)
 
 
 def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, shrinking=True, folds=None,
@@ -770,6 +812,8 @@ def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, s
     read from the double kernels, which is what libsvm computes for ``SVC(kernel='linear' | 'rbf')`` on features whose
     fp64 kernel values these are (see k_searchlight_kernels)."""
     lib = _lib.load()
+    if folds is not None and folds.wide:
+        raise ValueError("svm_cv_f64 takes make_svm_folds folds (at most 64 epochs)")
     if K_fit.dtype != torch.float64 or K_pred.dtype != torch.float64 or K_fit.shape != K_pred.shape \
             or K_fit.dim() != 3 or K_fit.shape[1] != K_fit.shape[2]:
         raise ValueError("K_fit and K_pred must be float64 [nv, E, E] of the same shape")

@@ -95,7 +95,7 @@ class VoxelSelector:
     gpu_cv: run the voxelwise cross validation on the GPU (batched restatement of libsvm's SMO, with or without its
         shrinking heuristic as ``clf.shrinking`` says, with the same iterations and decisions as scikit-learn; more than
         two conditions one-vs-one with libsvm's vote, see engine.svm_cv_precomputed) for
-        ``SVC(kernel='precomputed')`` on the kernel matrices, and for ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')``
+        ``SVC(kernel='precomputed')`` on the kernel matrices (at most 256 epochs and 64 folds), and for ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')``
         with ``gamma='auto'`` or a number on the normalised correlation vectors themselves: their fp64 kernel matrices
         are built on the GPU (engine.feature_kernels_f64, without the decimal shrink, as scikit-learn sees the features)
         and cross-validated by engine.svm_cv_f64 (at most 64 epochs and folds, no class weights, probability or tie
@@ -333,8 +333,9 @@ class VoxelSelector:
             K, k0 = mine, start
         else:
             k0 = 0
-        on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E)
-        folds = engine.make_svm_folds(self.labels, self.num_folds) if on_gpu else None
+        on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E,
+                                                         max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
+        folds = engine.svm_folds_for(self.labels, self.num_folds, E) if on_gpu else None
         results = []
         block = 8192
         for s in range(start, start + n, block):
@@ -387,8 +388,9 @@ class VoxelSelector:
         elif _is_precomputed_svc(clf):
             fused = engine.fused_supported(E, self.epochs_per_subj)
             block = self._plain_block(n)
-            on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E)
-            folds = engine.make_svm_folds(self.labels, self.num_folds) if on_gpu else None
+            on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E,
+                                                             max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
+            folds = engine.svm_folds_for(self.labels, self.num_folds, E) if on_gpu else None
             for s in range(start, start + n, block):
                 nb = min(block, start + n - s)
                 K = engine.voxel_kernels(rows_op, cols_op, s, nb, self.epochs_per_subj,

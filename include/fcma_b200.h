@@ -225,6 +225,15 @@ int fcma_svm_cv_solve(const float *K_dev, long nv, int E, int nproblems, const v
 int fcma_svm_cv_solve_f64(const double *K_fit_dev, const double *K_pred_dev, long nv, int E, int nproblems,
                           const void *folds_host, double C, double tol, int max_iter, int shrinking, int *correct_dev,
                           unsigned long long *bits_dev, int *iters_dev, void *stream);
+/* fcma_svm_cv_solve for wider problems, on float kernels [nv][E][E] with 2 <= E <= 256: folds_host points to nproblems
+ * structs SvmFoldWide {int n_train, n_pos, n_test, pad; int train_idx[256]; int test_idx[256];
+ * unsigned char test_pos[256]} (2320 bytes; 2 <= n_train <= 256, n_test <= 256, at most 4096 problems).  Bit t % 64 of
+ * bits_dev[(v*nproblems + p)*4 + t / 64] is set when sample test_idx[t] of problem p falls on the side of the first
+ * class (words past the held-out samples are 0).  Same iterations and decisions as fcma_svm_cv_solve on the same
+ * problems; Q is read from K_dev instead of a shared-memory copy, so it is the slower of the two at E <= 64. */
+int fcma_svm_cv_solve_wide(const float *K_dev, long nv, int E, int nproblems, const void *folds_host, double C,
+                           double tol, int max_iter, int shrinking, int *correct_dev, unsigned long long *bits_dev,
+                           int *iters_dev, void *stream);
 
 /* ---- searchlight kernel matrices (MVPAVoxelSelector, mvpa_voxelselector.py:34-49 per centre) --------------------------
  * vol_dev: float32 [nx][ny][nz][E] (epochs contiguous per voxel); mask_dev: bytes [nx][ny][nz]; shape_dev: bytes
