@@ -75,8 +75,12 @@ SIGNATURES = {
                                       c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_svm_cv_solve_wide": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double, c_int,
                                        c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_svm_cv_solve_f64_wide": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double,
+                                           ctypes.c_double, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_searchlight_kernels": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                          c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_searchlight_kernels_wide": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_int, c_void_p,
+                                              c_void_p, c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcma_voxel_feature_kernels": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_long, c_long, c_long, c_long, c_int,
                                            c_int, ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "fcma_gemm_nt": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_long, c_long, c_long, c_long,

@@ -4112,6 +4112,19 @@ extern "C" int fcma_svm_cv_solve_wide(const float *K_dev, long nv, int E, int np
     return svm_cv_impl<float, SvmFoldWide>("fcma_svm_cv_solve_wide", K_dev, nullptr, nv, E, nproblems, folds_host, C,
                                            tol, max_iter, shrinking, correct_dev, iters_dev, bits_dev, stream);
 }
+// fcma_svm_cv_solve_f64 for up to 256 epochs: SvmFoldWide problems, 4 decision words per problem, 4 or 8 slots per lane
+// as in fcma_svm_cv_solve_wide.
+extern "C" int fcma_svm_cv_solve_f64_wide(const double *K_fit_dev, const double *K_pred_dev, long nv, int E,
+                                          int nproblems, const void *folds_host, double C, double tol, int max_iter,
+                                          int shrinking, int *correct_dev, unsigned long long *bits_dev, int *iters_dev,
+                                          void *stream)
+{
+    if (!bits_dev && !correct_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64_wide: no output requested");
+    if (!K_pred_dev) return fail(FCMA_EINVAL, "fcma_svm_cv_solve_f64_wide: null K_pred");
+    return svm_cv_impl<double, SvmFoldWide>("fcma_svm_cv_solve_f64_wide", K_fit_dev, K_pred_dev, nv, E, nproblems,
+                                            folds_host, C, tol, max_iter, shrinking, correct_dev, iters_dev, bits_dev,
+                                            stream);
+}
 // Checks the fold problems (who: the entry point the messages name) and launches k_svm_cv on them: SvmFold problems
 // with NS = 2, SvmFoldWide problems with the fewest slots per lane that hold every problem
 template <typename KT, typename Fold>
@@ -4282,21 +4295,137 @@ __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float 
     }
 }
 
-extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E,
-                                        const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
-                                        const long *centres_host, long M, int kind, const double *gamma_host,
-                                        double *K_fit_dev, double *K_pred_dev, void *stream)
+// Tiled form for up to 256 epochs (fcma_searchlight_kernels_wide).  The [E][E] output is cut into SLT x SLT tiles, and
+// CTA (centre m, blockIdx.y) computes the upper tile (I, J), I <= J, from the row epochs [I SLT, I SLT + nr) and the
+// column epochs [J SLT, J SLT + nc) of the features, staged through shared memory in chunks of SL_CHUNK cube positions
+// (any radius).  Thread (tx, ty) of a 16 x 16 grid owns the entries (ty + 16u, tx + 16v), u, v < 4, and sums each one
+// exactly as k_searchlight_kernels sums a pair a <= b (cube order, every operation rounded separately), so an entry
+// depends on x_a and x_b only, never on E or on the tile.  rbf: threads 0..SLT-1 sum G_aa of the row epochs and threads
+// SLT..2 SLT-1 G_bb of the column epochs in the same order.  The tile goes out through shared memory in coalesced rows;
+// an off-diagonal tile also as its mirror image (J, I), and a diagonal tile stores its entries a <= b at (a, b) and
+// (b, a), so both matrices are exactly symmetric.
+#define SLT 64
+#define SLT_PITCH 65   // doubles per staged tile row: the mirror's column reads hit distinct bank pairs
+
+template <int KIND>
+__global__ void __launch_bounds__(SL_THREADS, 2)
+    k_searchlight_kernels_tiled(const float *__restrict__ vol, int ny, int nz, int E, const unsigned char *__restrict__ mask,
+                                int r, const unsigned char *__restrict__ shape, const long *__restrict__ centres,
+                                const double *__restrict__ gamma, double *__restrict__ K_fit, double *__restrict__ K_pred)
+{
+    __shared__ double s_tile[SLT * SLT_PITCH];        // the finished tile; the staged features while summing
+    __shared__ double s_diag[2][SLT];                 // rbf: G_aa of the row epochs, G_bb of the column epochs
+    __shared__ long s_vox[SL_CHUNK];                  // the chunk's cube positions: voxel index, or -1 if inactive
+    float *xr = reinterpret_cast<float *>(s_tile);    // [SL_CHUNK][SLT] row epochs
+    float *xc = xr + SL_CHUNK * SLT;                  // [SL_CHUNK][SLT] column epochs
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const long m = blockIdx.x;
+    const long c = centres[m];
+    const int cz = (int)(c % nz), cy = (int)((c / nz) % ny), cx = (int)(c / ((long)nz * ny));
+    const int side = 2 * r + 1, ncube = side * side * side;
+    // upper tile number t -> (I, J): tile row I holds the nt - I tiles (I, I..nt-1)
+    const int nt = (E + SLT - 1) / SLT;
+    int I = 0, t = blockIdx.y;
+    while (t >= nt - I) t -= nt - I++;
+    const int J = I + t;
+    const int r0 = I * SLT, c0 = J * SLT, nr = min(SLT, E - r0), nc = min(SLT, E - c0);
+
+    double g[4][4], d[4][4], gd = 0.0;
+#pragma unroll
+    for (int u = 0; u < 4; u++)
+#pragma unroll
+        for (int v = 0; v < 4; v++) g[u][v] = d[u][v] = 0.0;
+
+    for (int o0 = 0; o0 < ncube; o0 += SL_CHUNK) {
+        const int nch = min(SL_CHUNK, ncube - o0);
+        __syncthreads();
+        if (tid < nch) {
+            const int o = o0 + tid;
+            const int i = o / (side * side), j = (o / side) % side, k = o % side;
+            const long vox = ((long)(cx - r + i) * ny + (cy - r + j)) * nz + (cz - r + k);
+            s_vox[tid] = shape[o] && mask[vox] ? vox : -1;
+        }
+        __syncthreads();
+        for (int idx = tid; idx < nch * 2 * SLT; idx += SL_THREADS) {
+            const int q = idx / (2 * SLT), e = idx % (2 * SLT);
+            const bool row = e < SLT;
+            const int ee = row ? e : e - SLT, n = row ? nr : nc;
+            const long vox = s_vox[q];
+            (row ? xr : xc)[q * SLT + ee] = vox >= 0 && ee < n ? vol[vox * E + (row ? r0 : c0) + ee] : 0.f;
+        }
+        __syncthreads();
+        for (int q = 0; q < nch; q++) {
+            if (s_vox[q] < 0) continue;
+            const float *xq_r = xr + q * SLT, *xq_c = xc + q * SLT;
+            double xa[4], xb[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) xa[u] = (double)xq_r[ty + 16 * u];
+#pragma unroll
+            for (int v = 0; v < 4; v++) xb[v] = (double)xq_c[tx + 16 * v];
+#pragma unroll
+            for (int u = 0; u < 4; u++)
+#pragma unroll
+                for (int v = 0; v < 4; v++) {
+                    g[u][v] = __dadd_rn(g[u][v], __dmul_rn(xa[u], xb[v]));
+                    if (KIND == 1) {
+                        const double df = __dsub_rn(xa[u], xb[v]);
+                        d[u][v] = __dadd_rn(d[u][v], __dmul_rn(df, df));
+                    }
+                }
+            if (KIND == 1 && tid < 2 * SLT) {
+                const double x = (double)(tid < SLT ? xq_r[tid] : xq_c[tid - SLT]);
+                gd = __dadd_rn(gd, __dmul_rn(x, x));
+            }
+        }
+    }
+
+    if (KIND == 1 && tid < 2 * SLT) s_diag[tid / SLT][tid % SLT] = gd;
+    const double gm = KIND == 1 ? gamma[m] : 0.0;
+    double *const out[2] = {K_fit + (size_t)m * E * E, K_pred + (size_t)m * E * E};
+#pragma unroll
+    for (int pass = 0; pass < (KIND == 1 ? 2 : 1); pass++) {
+        __syncthreads();      // the staged features (pass 0) or the previous tile (pass 1) are no longer read
+#pragma unroll
+        for (int u = 0; u < 4; u++)
+#pragma unroll
+            for (int v = 0; v < 4; v++) {
+                const int a = ty + 16 * u, b = tx + 16 * v;
+                if (a >= nr || b >= nc || (I == J && a > b)) continue;
+                double val = g[u][v];
+                if (KIND == 1) val = pass == 0 ? rbf_fit(gm, s_diag[0][a], s_diag[1][b], g[u][v]) : rbf_pred(gm, d[u][v]);
+                s_tile[a * SLT_PITCH + b] = val;
+                if (I == J) s_tile[b * SLT_PITCH + a] = val;
+            }
+        __syncthreads();
+        double *K = out[pass];
+        for (int idx = tid; idx < nr * nc; idx += SL_THREADS) {
+            const int a = idx / nc, b = idx - a * nc;
+            K[(size_t)(r0 + a) * E + c0 + b] = s_tile[a * SLT_PITCH + b];
+        }
+        if (I != J)
+            for (int idx = tid; idx < nr * nc; idx += SL_THREADS) {
+                const int b = idx / nr, a = idx - b * nr;
+                K[(size_t)(c0 + b) * E + r0 + a] = s_tile[a * SLT_PITCH + b];
+            }
+    }
+}
+
+// The argument checks of the searchlight entry points (who: the entry point the messages name; 1 <= E <= e_max), and
+// the centres (and, for rbf, the gammas) copied to the device
+static int searchlight_args(const char *who, int e_max, const float *vol_dev, long nx, long ny, long nz, int E,
+                            const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
+                            const long *centres_host, long M, int kind, const double *gamma_host, double *K_fit_dev,
+                            double *K_pred_dev, cudaStream_t st, AsyncBuf &cbuf, AsyncBuf &gbuf)
 {
     int rc = check_device();
     if (rc) return rc;
     if (!vol_dev || !mask_dev || !shape_dev || !centres_host || !K_fit_dev || M <= 0 || nx <= 0 || ny <= 0 || nz <= 0)
-        return fail(FCMA_EINVAL, "fcma_searchlight_kernels: null buffer or empty volume / centre list");
-    if (E < 1 || E > 64) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: E = %d outside 1..64", E);
-    if (sl_rad < 0) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: negative sl_rad");
-    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: kind must be 0 (linear) or 1 (rbf)");
-    if (kind == 1 && (!gamma_host || !K_pred_dev))
-        return fail(FCMA_EINVAL, "fcma_searchlight_kernels: rbf needs gamma and K_pred");
-    if (M > 0x7fffffffL) return fail(FCMA_EINVAL, "fcma_searchlight_kernels: too many centres in one call");
+        return fail(FCMA_EINVAL, "%s: null buffer or empty volume / centre list", who);
+    if (E < 1 || E > e_max) return fail(FCMA_EINVAL, "%s: E = %d outside 1..%d", who, E, e_max);
+    if (sl_rad < 0) return fail(FCMA_EINVAL, "%s: negative sl_rad", who);
+    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "%s: kind must be 0 (linear) or 1 (rbf)", who);
+    if (kind == 1 && (!gamma_host || !K_pred_dev)) return fail(FCMA_EINVAL, "%s: rbf needs gamma and K_pred", who);
+    if (M > 0x7fffffffL) return fail(FCMA_EINVAL, "%s: too many centres in one call", who);
     for (long m = 0; m < M; m++) {
         const long c = centres_host[m];
         if (c < 0 || c >= nx * ny * nz) return fail(FCMA_EINVAL, "centre %ld: index %ld outside the volume", m, c);
@@ -4304,14 +4433,25 @@ extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, 
         if (x < sl_rad || y < sl_rad || z < sl_rad || x >= nx - sl_rad || y >= ny - sl_rad || z >= nz - sl_rad)
             return fail(FCMA_EINVAL, "centre %ld (%ld, %ld, %ld) is closer than sl_rad = %d to a face", m, x, y, z, sl_rad);
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    AsyncBuf cbuf, gbuf;
     CUDA_TRY(cbuf.alloc(sizeof(long) * M, st));
     CUDA_TRY(cudaMemcpyAsync(cbuf.p, centres_host, sizeof(long) * M, cudaMemcpyHostToDevice, st));
     if (kind == 1) {
         CUDA_TRY(gbuf.alloc(sizeof(double) * M, st));
         CUDA_TRY(cudaMemcpyAsync(gbuf.p, gamma_host, sizeof(double) * M, cudaMemcpyHostToDevice, st));
     }
+    return FCMA_OK;
+}
+
+extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E,
+                                        const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
+                                        const long *centres_host, long M, int kind, const double *gamma_host,
+                                        double *K_fit_dev, double *K_pred_dev, void *stream)
+{
+    cudaStream_t st = (cudaStream_t)stream;
+    AsyncBuf cbuf, gbuf;
+    int rc = searchlight_args("fcma_searchlight_kernels", 64, vol_dev, nx, ny, nz, E, mask_dev, sl_rad, shape_dev,
+                              centres_host, M, kind, gamma_host, K_fit_dev, K_pred_dev, st, cbuf, gbuf);
+    if (rc) return rc;
     const size_t smem = (size_t)E * E * sizeof(double) + E * sizeof(double) + SL_CHUNK * E * sizeof(float) + SL_CHUNK;
     const long *cdev = static_cast<const long *>(cbuf.p);
     const double *gdev = static_cast<const double *>(gbuf.p);
@@ -4320,6 +4460,28 @@ extern "C" int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, 
                              vol_dev, (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev,
                              K_pred_dev);
     return launch_kernel(k_searchlight_kernels<1>, (unsigned)M, SL_THREADS, smem, st, "k_searchlight_kernels", vol_dev,
+                         (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev, K_pred_dev);
+}
+
+extern "C" int fcma_searchlight_kernels_wide(const float *vol_dev, long nx, long ny, long nz, int E,
+                                             const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
+                                             const long *centres_host, long M, int kind, const double *gamma_host,
+                                             double *K_fit_dev, double *K_pred_dev, void *stream)
+{
+    cudaStream_t st = (cudaStream_t)stream;
+    AsyncBuf cbuf, gbuf;
+    int rc = searchlight_args("fcma_searchlight_kernels_wide", 256, vol_dev, nx, ny, nz, E, mask_dev, sl_rad, shape_dev,
+                              centres_host, M, kind, gamma_host, K_fit_dev, K_pred_dev, st, cbuf, gbuf);
+    if (rc) return rc;
+    const int nt = (E + SLT - 1) / SLT;
+    const dim3 grid((unsigned)M, nt * (nt + 1) / 2);
+    const long *cdev = static_cast<const long *>(cbuf.p);
+    const double *gdev = static_cast<const double *>(gbuf.p);
+    if (kind == 0)
+        return launch_kernel(k_searchlight_kernels_tiled<0>, grid, SL_THREADS, 0, st, "k_searchlight_kernels_tiled",
+                             vol_dev, (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev,
+                             K_fit_dev);
+    return launch_kernel(k_searchlight_kernels_tiled<1>, grid, SL_THREADS, 0, st, "k_searchlight_kernels_tiled", vol_dev,
                          (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev, K_pred_dev);
 }
 

@@ -632,12 +632,13 @@ def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True, max_epochs
     return True
 
 
-def svc_feature_kind(clf, labels, num_folds, E):
+def svc_feature_kind(clf, labels, num_folds, E, max_epochs=64):
     """``'linear'`` / ``'rbf'`` if ``cross_val_score(clf, X, labels, cv=StratifiedKFold(num_folds))`` on float32
     features ``X`` (E samples) can be computed as ``svm_cv_f64`` on the fp64 kernel matrices of ``X``, else None:
     ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')`` with ``gamma='auto'`` or a number >= 0, without class weights,
-    probability or tie breaking, E <= 64, at most 64 folds that ``make_svm_folds`` accepts.  ``gamma='scale'`` depends on
-    the variance of the training features and stays with scikit-learn."""
+    probability or tie breaking, E <= ``max_epochs`` (64, or up to ``SVM_WIDE_MAX_EPOCHS``, solved with
+    ``svm_folds_for`` folds), at most 64 folds that ``svm_folds_for`` accepts.  ``gamma='scale'`` depends on the variance
+    of the training features and stays with scikit-learn."""
     import numbers
     import sklearn.svm
     if not isinstance(clf, sklearn.svm.SVC):
@@ -652,10 +653,10 @@ def svc_feature_kind(clf, labels, num_folds, E):
     # scikit-learn >= 1.9 uses the string 'deprecated' as the default of `probability`
     if clf.class_weight is not None or getattr(clf, 'probability', False) is True or getattr(clf, 'break_ties', False):
         return None
-    if E > 64 or num_folds > 64:
+    if E > min(max_epochs, SVM_WIDE_MAX_EPOCHS) or num_folds > 64:
         return None
     try:
-        make_svm_folds(labels, num_folds)
+        svm_folds_for(labels, num_folds, E)
     except ValueError:
         return None
     return kind
@@ -810,17 +811,18 @@ def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, s
     """``svm_cv_precomputed`` on fp64 kernels: ``K_fit`` / ``K_pred`` float64 CUDA ``[nv, E, E]`` (``K_pred`` may be
     ``K_fit``).  The solver keeps Q in float and QD, the gradient and the decisions in double with QD and the decisions
     read from the double kernels, which is what libsvm computes for ``SVC(kernel='linear' | 'rbf')`` on features whose
-    fp64 kernel values these are (see k_searchlight_kernels)."""
+    fp64 kernel values these are (see k_searchlight_kernels).  The form of ``folds`` picks the solver:
+    ``make_svm_folds`` problems (the default, at most 64 epochs) run fcma_svm_cv_solve_f64, ``make_svm_folds_wide`` /
+    ``svm_folds_for`` problems fcma_svm_cv_solve_f64_wide (up to ``SVM_WIDE_MAX_EPOCHS``)."""
     lib = _lib.load()
-    if folds is not None and folds.wide:
-        raise ValueError("svm_cv_f64 takes make_svm_folds folds (at most 64 epochs)")
     if K_fit.dtype != torch.float64 or K_pred.dtype != torch.float64 or K_fit.shape != K_pred.shape \
             or K_fit.dim() != 3 or K_fit.shape[1] != K_fit.shape[2]:
         raise ValueError("K_fit and K_pred must be float64 [nv, E, E] of the same shape")
     if not (K_fit.is_contiguous() and K_pred.is_contiguous()):
         raise ValueError("K_fit and K_pred must be contiguous")
-    return _svm_cv(lib.fcma_svm_cv_solve_f64, (_ptr(K_fit), _ptr(K_pred)), K_fit, labels, num_folds, C, tol, max_iter,
-                   shrinking, folds, return_iters)
+    solve = lib.fcma_svm_cv_solve_f64_wide if folds is not None and folds.wide else lib.fcma_svm_cv_solve_f64
+    return _svm_cv(solve, (_ptr(K_fit), _ptr(K_pred)), K_fit, labels, num_folds, C, tol, max_iter, shrinking, folds,
+                   return_iters)
 
 
 # ------------------------------------------------------------------ searchlight (MVPAVoxelSelector)
@@ -860,10 +862,22 @@ def searchlight_used_voxels(mask, centres, sl_rad, shape):
 
 def searchlight_kernels(vol, mask, sl_rad, shape, centres, kind="linear", gamma=None):
     """fp64 kernel matrices of searchlight centres (k_searchlight_kernels): ``vol`` float32 CUDA ``[X, Y, Z, E]``,
-    ``mask`` / ``shape`` uint8 (or bool) CUDA volumes, ``centres`` int64 host indices (``searchlight_centres``).
-    ``kind='linear'``: returns ``(G, G)``; ``kind='rbf'`` with one ``gamma`` per centre: ``(K_fit, K_pred)``, the
-    x_square form libsvm trains with and the difference form its decisions use.  Both float64 ``[M, E, E]``."""
-    lib = _lib.load()
+    1 <= E <= 64, ``mask`` / ``shape`` uint8 (or bool) CUDA volumes, ``centres`` int64 host indices
+    (``searchlight_centres``).  ``kind='linear'``: returns ``(G, G)``; ``kind='rbf'`` with one ``gamma`` per centre:
+    ``(K_fit, K_pred)``, the x_square form libsvm trains with and the difference form its decisions use.  Both float64
+    ``[M, E, E]``."""
+    return _searchlight_kernels(_lib.load().fcma_searchlight_kernels, vol, mask, sl_rad, shape, centres, kind, gamma)
+
+
+def searchlight_kernels_wide(vol, mask, sl_rad, shape, centres, kind="linear", gamma=None):
+    """``searchlight_kernels`` for 1 <= E <= 256 (k_searchlight_kernels_tiled): the same arguments and outputs, and
+    every entry the value ``searchlight_kernels`` gives for the same two epochs' features."""
+    return _searchlight_kernels(_lib.load().fcma_searchlight_kernels_wide, vol, mask, sl_rad, shape, centres, kind,
+                                gamma)
+
+
+def _searchlight_kernels(entry, vol, mask, sl_rad, shape, centres, kind, gamma):
+    """The body of searchlight_kernels and searchlight_kernels_wide around one call of the C entry point ``entry``."""
     if vol.dim() != 4 or vol.dtype != torch.float32 or not vol.is_contiguous():
         raise ValueError("vol must be a contiguous float32 [X, Y, Z, E] tensor")
     X, Y, Z, E = vol.shape
@@ -892,8 +906,7 @@ def searchlight_kernels(vol, mask, sl_rad, shape, centres, kind="linear", gamma=
     K_fit = torch.empty((M, E, E), dtype=torch.float64, device=vol.device)
     K_pred = K_fit if kcode == 0 else torch.empty_like(K_fit)
     with torch.cuda.device(vol.device):
-        _lib.check(lib.fcma_searchlight_kernels(_ptr(vol), X, Y, Z, E, _ptr(mask), int(sl_rad), _ptr(shape),
-                                                c.ctypes.data_as(ctypes.c_void_p), M, kcode,
-                                                g.ctypes.data_as(ctypes.c_void_p) if g is not None else None,
-                                                _ptr(K_fit), _ptr(K_pred) if kcode == 1 else None, _stream_ptr()))
+        _lib.check(entry(_ptr(vol), X, Y, Z, E, _ptr(mask), int(sl_rad), _ptr(shape), c.ctypes.data_as(ctypes.c_void_p),
+                         M, kcode, g.ctypes.data_as(ctypes.c_void_p) if g is not None else None, _ptr(K_fit),
+                         _ptr(K_pred) if kcode == 1 else None, _stream_ptr()))
     return K_fit, K_pred

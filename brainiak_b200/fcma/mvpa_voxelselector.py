@@ -6,11 +6,12 @@ accuracy of ``clf`` on the centre's features (the voxels of its cube inside both
 in C order), and ``run(clf)`` returns ``(result_volume, results)`` as the reference does.
 
 For ``SVC(kernel='linear')`` and ``SVC(kernel='rbf')`` with ``gamma='auto'`` or a number, both stages run on the
-GPU: k_searchlight_kernels builds each centre's fp64 kernel matrices and the batched libsvm SMO restatement
-cross-validates them in fp64 (engine.svm_cv_f64).  libsvm keeps Q in float but QD and the decision values in double,
-so fp64 kernels give the same iterations and predictions as scikit-learn on the features (DESIGN.md).  Any other
-classifier (``gamma='scale'``, poly, sigmoid, other estimators), float64 data, more than 64 epochs, folds the solver
-cannot express or ``gpu_cv=False`` run the reference's per-centre ``cross_val_score`` on the host.
+GPU for up to 256 epochs: k_searchlight_kernels (k_searchlight_kernels_tiled above 32 epochs) builds each centre's fp64
+kernel matrices and the batched libsvm SMO restatement cross-validates them in fp64 (engine.svm_cv_f64, on
+``engine.svm_folds_for`` folds: its wide form above 64 epochs).  libsvm keeps Q in float but QD and the decision values
+in double, so fp64 kernels give the same iterations and predictions as scikit-learn on the features (DESIGN.md).  Any
+other classifier (``gamma='scale'``, poly, sigmoid, other estimators), float64 data, more than 256 epochs, folds the
+solver cannot express or ``gpu_cv=False`` run the reference's per-centre ``cross_val_score`` on the host.
 """
 import logging
 
@@ -58,8 +59,10 @@ class MVPAVoxelSelector:
     Keyword-only extensions
     -----------------------
     device: CUDA device (default: the current one)
-    gpu_cv: score eligible SVC classifiers on the GPU (default); ``False`` -> the reference's host loop
-    batch_centres: centres per GPU batch (default: sized to free device memory)
+    gpu_cv: score eligible SVC classifiers on the GPU (default; up to 256 epochs); ``False`` -> the reference's host
+        loop
+    batch_centres: centres per GPU batch (default: sized to free device memory; a centre's kernel matrices take
+        8 E^2 bytes, twice that for rbf)
     """
 
     def __init__(self, data, mask, labels, num_folds, sl, *, device=None, gpu_cv=True, batch_centres=None):
@@ -82,7 +85,8 @@ class MVPAVoxelSelector:
         """'linear' / 'rbf' if ``clf`` and the data can be scored on the GPU, else None."""
         if not self.gpu_cv:
             return None
-        kind = engine.svc_feature_kind(clf, self.labels, self.num_folds, self.data.shape[3])
+        kind = engine.svc_feature_kind(clf, self.labels, self.num_folds, self.data.shape[3],
+                                       max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
         if kind is not None and np.asarray(self.data).dtype != np.float32:
             logger.info('MVPAVoxelSelector: data is %s, not float32: scoring on the host', np.asarray(self.data).dtype)
             return None
@@ -171,7 +175,10 @@ class MVPAVoxelSelector:
             raise ValueError('the data holds NaN or infinity in voxels the searchlight uses')
         dev = self._torch_device()
         E = data.shape[3]
-        folds = engine.make_svm_folds(self.labels, self.num_folds)
+        folds = engine.svm_folds_for(self.labels, self.num_folds, E)
+        # both builders give the same bytes; the untiled one is faster up to 32 epochs, the tiled one from 64 on (DESIGN.md
+        # §3.7), and only the tiled one goes past 64
+        kernels = engine.searchlight_kernels_wide if E > 32 else engine.searchlight_kernels
         if kind == 'rbf':
             gamma = 1.0 / nfeat.astype(np.float64) if clf.gamma == 'auto' else np.full(len(centres), float(clf.gamma))
         with torch.cuda.device(dev):
@@ -187,8 +194,7 @@ class MVPAVoxelSelector:
             acc = []
             for b0 in range(0, len(centres), batch):
                 cb = centres[b0:b0 + batch]
-                K_fit, K_pred = engine.searchlight_kernels(vol, mask_d, r, shape_d, cb, kind,
-                                                           gamma[b0:b0 + batch] if kind == 'rbf' else None)
+                K_fit, K_pred = kernels(vol, mask_d, r, shape_d, cb, kind, gamma[b0:b0 + batch] if kind == 'rbf' else None)
                 acc.append(engine.svm_cv_f64(K_fit, K_pred, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
                                              max_iter=clf.max_iter, shrinking=clf.shrinking, folds=folds))
                 del K_fit, K_pred

@@ -234,6 +234,12 @@ int fcma_svm_cv_solve_f64(const double *K_fit_dev, const double *K_pred_dev, lon
 int fcma_svm_cv_solve_wide(const float *K_dev, long nv, int E, int nproblems, const void *folds_host, double C,
                            double tol, int max_iter, int shrinking, int *correct_dev, unsigned long long *bits_dev,
                            int *iters_dev, void *stream);
+/* fcma_svm_cv_solve_f64 for wider problems, on fp64 kernels [nv][E][E] with 2 <= E <= 256: SvmFoldWide problems and four
+ * decision words per problem, as in fcma_svm_cv_solve_wide.  Same iterations and decisions as fcma_svm_cv_solve_f64 on
+ * the same problems. */
+int fcma_svm_cv_solve_f64_wide(const double *K_fit_dev, const double *K_pred_dev, long nv, int E, int nproblems,
+                               const void *folds_host, double C, double tol, int max_iter, int shrinking,
+                               int *correct_dev, unsigned long long *bits_dev, int *iters_dev, void *stream);
 
 /* ---- searchlight kernel matrices (MVPAVoxelSelector, mvpa_voxelselector.py:34-49 per centre) --------------------------
  * vol_dev: float32 [nx][ny][nz][E] (epochs contiguous per voxel); mask_dev: bytes [nx][ny][nz]; shape_dev: bytes
@@ -244,6 +250,12 @@ int fcma_svm_cv_solve_wide(const float *K_dev, long nv, int E, int nproblems, co
 int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E, const unsigned char *mask_dev,
                              int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, int kind,
                              const double *gamma_host, double *K_fit_dev, double *K_pred_dev, void *stream);
+/* fcma_searchlight_kernels for 1 <= E <= 256: the same arguments and outputs, computed in 64 x 64 tiles.  Every entry is
+ * summed in the same order as fcma_searchlight_kernels sums it, so it depends only on the two epochs' features: the
+ * entries of a subset S of the epochs equal fcma_searchlight_kernels on the volume of those epochs, bit for bit. */
+int fcma_searchlight_kernels_wide(const float *vol_dev, long nx, long ny, long nz, int E, const unsigned char *mask_dev,
+                                  int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, int kind,
+                                  const double *gamma_host, double *K_fit_dev, double *K_pred_dev, void *stream);
 
 /* ---- per-voxel fp64 kernels of the normalised correlation vectors (VoxelSelector with SVC(kernel='linear' | 'rbf')) ----
  * The plain pipeline of fcma_voxel_kernels (one or two masks, same operands, work buffer and passes) with a different
