@@ -3044,15 +3044,19 @@ static bool half_block(int precision, int flags)
     return half;
 }
 
-// Second stage of fcma_voxel_feature_kernels: the per-voxel fp64 kernel matrices of the normalised correlation vectors
-// (k_norm_gram_f64) instead of the fp32 SYRK.  kind 0 linear, 1 rbf; outputs [nb][E][E].
+// Second stage of fcma_voxel_feature_kernels (E <= 64: k_norm_gram_f64) and fcma_voxel_feature_kernels_wide (tiled:
+// E <= 256): the per-voxel fp64 kernel matrices of the normalised correlation vectors instead of the fp32 SYRK.  kind 0
+// linear, 1 rbf; outputs [nb][E][E].
 struct FeatureStage {
     int kind;
     double gamma;
     double *K_fit, *K_pred;
+    bool tiled;
 };
 static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
                                 cudaStream_t st);
+static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
+                                     cudaStream_t st);
 
 // shared body of the fused pipelines; with `feat` the GEMM writes raw r and the feature stage replaces normalise+SYRK
 static int run_pipeline(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2, long start,
@@ -3095,8 +3099,8 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
         const float beta = sum_over_rows ? 1.0f : 0.0f;
         if (feat) {
             const size_t off = (size_t)done * E * E;
-            rc = launch_norm_gram_f64(C, eps, feat->kind, feat->gamma, feat->K_fit + off,
-                                      feat->K_pred ? feat->K_pred + off : nullptr, st);
+            rc = (feat->tiled ? launch_feature_gram_tiled : launch_norm_gram_f64)(
+                C, eps, feat->kind, feat->gamma, feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st);
         } else if (tiled || (normalise && fused)) {
             rc = launch_norm_syrk(C, normalise ? eps : 0, (normalise && fisher_in_gemm) ? 1 : 0,
                                   mask_self ? start + done : -1, beta, Kdst, sum_over_rows, st);
@@ -4675,21 +4679,265 @@ static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double ga
     return ok ? rc : fail(FCMA_EINVAL, "internal: no k_norm_gram_f64 instantiation for E=%d", E);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Tiled form for up to 256 epochs (fcma_voxel_feature_kernels_wide), in two or three launches over the raw block:
+//   k_block_within_subject_norm  z = within_subject_column(r) in place, tiled or strided block (a subject may straddle
+//                                the 64-epoch tiles, so the whole column is normalised before any tile reads it)
+//   k_feature_gram_tiled<KIND>   CTA (row i, upper FGT x FGT tile (I, J), I <= J) streams the row epochs
+//                                [I FGT, I FGT + nr) and the column epochs [J FGT, J FGT + nc) of z through shared memory
+//                                in chunks of NG_CH columns, widened to fp64 transposed [NG_CH][FG_LDT].
+//                                G: warp w owns the tile's row block w of 8 epochs against the column blocks 0..7 (a
+//                                diagonal tile: w..7), one mma.sync m8n8k4 per block and k-step, the k-steps in column
+//                                order: every entry is summed in the same order in every tile, whatever its E.
+//                                D (rbf): thread (ty, tx) of a 16 x 16 grid owns (ty + 16u, tx + 16v), u, v < 4 (a
+//                                diagonal tile: ty <= tx on 136 threads, as k_norm_gram_f64), each summed sequentially
+//                                over j with the difference then one fma, exactly as k_norm_gram_f64 sums it.
+//                                The tile goes out through shared memory in coalesced rows; an off-diagonal tile also
+//                                as its mirror (J, I), a diagonal tile stores its entries a <= b at (a, b) and (b, a), so
+//                                both matrices are exactly symmetric.  rbf: K_fit holds G and K_pred holds D.
+//   k_feature_rbf_epilogue       rbf: K_fit = rbf_fit(G_aa, G_bb, G_ab), K_pred = rbf_pred(D) in place, per row (G_aa
+//                                comes from other CTAs' diagonal tiles).  K_fit_aa = K_pred_aa = 1 exactly.
+// No atomics: two runs are bit-identical.
+#define FGT 64
+#define FG_LDT (FGT + 4)     // doubles per staged column: conflict-free widening, MMA fragments and D reads
+#define FG_PITCH 65          // doubles per row of the staged output tile: the mirror's column reads hit distinct banks
+
+// element (i, e, j) of a CorrBlock, as (row pointer) + e * ld + col_off(j)
+__device__ __forceinline__ long block_row_off(long i, long stride_i, long chunk_step, long t256)
+{
+    return chunk_step != 256 ? (i / 256) * t256 * chunk_step + (i % 256) * stride_i : i * stride_i;
+}
+
+__global__ void __launch_bounds__(256) k_block_within_subject_norm(float *C, long nb, int E, long n2, long stride_i,
+                                                                   long ld, long chunk_step, long t256, int eps)
+{
+    const long nsubj = E / eps;
+    const long total = nb * nsubj * n2;
+    for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
+        const long j = idx % n2, v = idx / n2, s = v % nsubj, i = v / nsubj;
+        within_subject_column(C + block_row_off(i, stride_i, chunk_step, t256) + (j / 256) * chunk_step + j % 256, ld, s,
+                              eps);
+    }
+}
+
+// rbf needs 16 G + 16 D sums and the next chunk per thread: one CTA per SM keeps them in registers without spills
+template <int KIND>
+__global__ void __launch_bounds__(NG_THREADS, KIND == 1 ? 1 : 2)
+    k_feature_gram_tiled(const float *__restrict__ Z, int E, long n2, long stride_i, long ld, long chunk_step, long t256,
+                         double *__restrict__ K_fit, double *__restrict__ K_pred)
+{
+    extern __shared__ double s_fg[];
+    double *zr = s_fg;                    // [NG_CH][FG_LDT] row epochs; then the [FGT][FG_PITCH] output tile
+    double *zc = zr + NG_CH * FG_LDT;     // [NG_CH][FG_LDT] column epochs (a diagonal tile reads zr)
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int nt = (E + FGT - 1) / FGT, ntiles = nt * (nt + 1) / 2;
+    const long i = blockIdx.x / ntiles;
+    int I = 0, tt = (int)(blockIdx.x % ntiles);
+    while (tt >= nt - I) tt -= nt - I++;
+    const int J = I + tt;
+    const bool diag = I == J;
+    const int r0 = I * FGT, c0 = J * FGT, nr = min(FGT, E - r0), nc = min(FGT, E - c0);
+    const double *zcol = diag ? zr : zc;
+    const float *Zi = Z + block_row_off(i, stride_i, chunk_step, t256);
+
+    // D: thread (ty, tx); a diagonal tile uses the 136 threads with ty <= tx
+    int ty = tid >> 4, tx = tid & 15;
+    if (diag) {
+        int q = tid;
+        ty = 0;
+        while (q >= 16 - ty && ty < 16) q -= 16 - ty++;
+        tx = ty + q;
+    }
+    const bool dq = KIND == 1 && (!diag || tid < 136);
+
+    // the thread stages epochs e + 32h (e = 4 warp + lane % 4) of both sets (row / column epochs) at the chunk's columns
+    // 8m + g: each warp reads 4 epochs x 8 columns per load (whole 32-byte sectors) and writes distinct banks of zr / zc
+    const int e0 = warp * 4 + t;
+    const float *src0[2][2];
+    bool elive[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        src0[0][h] = Zi + (long)(r0 + e0 + 32 * h) * ld + g;
+        src0[1][h] = Zi + (long)(c0 + e0 + 32 * h) * ld + g;
+        elive[0][h] = e0 + 32 * h < nr;
+        elive[1][h] = !diag && e0 + 32 * h < nc;
+    }
+    float pf[2][2][8];
+    auto prefetch = [&](long j0) {
+        const long off = (j0 / 256) * chunk_step + j0 % 256;
+#pragma unroll
+        for (int s = 0; s < 2; s++)
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int m = 0; m < 8; m++)
+                    pf[s][h][m] = elive[s][h] && j0 + 8 * m + g < n2 ? __ldg(src0[s][h] + off + 8 * m) : 0.f;
+    };
+
+    double acc[8][2];
+    double dacc[4][4];
+#pragma unroll
+    for (int v = 0; v < 8; v++) acc[v][0] = acc[v][1] = 0.0;
+#pragma unroll
+    for (int u = 0; u < 4; u++)
+#pragma unroll
+        for (int v = 0; v < 4; v++) dacc[u][v] = 0.0;
+
+    prefetch(0);
+    for (long j0 = 0; j0 < n2; j0 += NG_CH) {
+        __syncthreads();   // the previous chunk is consumed
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int m = 0; m < 8; m++) {
+                zr[(8 * m + g) * FG_LDT + e0 + 32 * h] = (double)pf[0][h][m];
+                if (!diag) zc[(8 * m + g) * FG_LDT + e0 + 32 * h] = (double)pf[1][h][m];
+            }
+        if (j0 + NG_CH < n2) prefetch(j0 + NG_CH);
+        __syncthreads();
+        for (int ks = 0; ks < NG_CH / 4; ks++) {
+            const double fa = zr[(ks * 4 + t) * FG_LDT + warp * 8 + g];
+            const double *zk = zcol + (ks * 4 + t) * FG_LDT + g;
+#pragma unroll
+            for (int v = 0; v < 8; v++)
+                if (!diag || v >= warp) dmma_m8n8k4(acc[v], fa, zk[v * 8]);
+        }
+        if (dq) {
+            for (int c = 0; c < NG_CH; c++) {
+                const double *za = zr + c * FG_LDT, *zb = zcol + c * FG_LDT;
+                double xa[4], xb[4];
+#pragma unroll
+                for (int u = 0; u < 4; u++) xa[u] = za[ty + 16 * u], xb[u] = zb[tx + 16 * u];
+#pragma unroll
+                for (int u = 0; u < 4; u++)
+#pragma unroll
+                    for (int v = 0; v < 4; v++) {
+                        const double df = __dsub_rn(xa[u], xb[v]);
+                        dacc[u][v] = __fma_rn(df, df, dacc[u][v]);
+                    }
+            }
+        }
+    }
+
+    double *tile = zr;
+    const size_t base = (size_t)i * E * E;
+#pragma unroll
+    for (int pass = 0; pass < (KIND == 1 ? 2 : 1); pass++) {
+        __syncthreads();   // the staged chunk (pass 0) or the previous tile (pass 1) is no longer read
+        if (pass == 0) {
+#pragma unroll
+            for (int v = 0; v < 8; v++) {
+                if (diag && v < warp) continue;
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int a = warp * 8 + g, b = v * 8 + 2 * t + h;
+                    if (diag && a > b) continue;
+                    tile[a * FG_PITCH + b] = acc[v][h];
+                    if (diag) tile[b * FG_PITCH + a] = acc[v][h];
+                }
+            }
+        } else if (dq) {
+#pragma unroll
+            for (int u = 0; u < 4; u++)
+#pragma unroll
+                for (int v = 0; v < 4; v++) {
+                    tile[(ty + 16 * u) * FG_PITCH + tx + 16 * v] = dacc[u][v];
+                    if (diag) tile[(tx + 16 * v) * FG_PITCH + ty + 16 * u] = dacc[u][v];
+                }
+        }
+        __syncthreads();
+        double *K = (pass == 0 ? K_fit : K_pred) + base;
+        for (int idx = tid; idx < nr * nc; idx += NG_THREADS) {
+            const int a = idx / nc, b = idx - a * nc;
+            K[(size_t)(r0 + a) * E + c0 + b] = tile[a * FG_PITCH + b];
+        }
+        if (!diag)
+            for (int idx = tid; idx < nr * nc; idx += NG_THREADS) {
+                const int b = idx / nr, a = idx - b * nr;
+                K[(size_t)(c0 + b) * E + r0 + a] = tile[a * FG_PITCH + b];
+            }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_feature_rbf_epilogue(int E, double gamma, double *__restrict__ K_fit,
+                                                              double *__restrict__ K_pred)
+{
+    __shared__ double s_diag[256];
+    const size_t base = (size_t)blockIdx.x * E * E;
+    for (int a = threadIdx.x; a < E; a += blockDim.x) s_diag[a] = K_fit[base + (size_t)a * E + a];
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < E * E; idx += blockDim.x) {
+        const int a = idx / E, b = idx - a * E;
+        K_fit[base + idx] = rbf_fit(gamma, s_diag[a], s_diag[b], K_fit[base + idx]);
+        K_pred[base + idx] = rbf_pred(gamma, K_pred[base + idx]);
+    }
+}
+
+// over the raw fp32 correlation block C, tiled or strided; normalises C in place
+static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
+                                     cudaStream_t st)
+{
+    const int E = C.E;
+    const long nb = C.rows;
+    if (C.rc) return C.rc;
+    if (E < 1 || E > 256 || eps < 1 || C.fp16) return fail(FCMA_EINVAL, "internal: k_feature_gram_tiled needs 1 <= E <= 256, eps >= 1, fp32");
+    float *Z = static_cast<float *>(C.base);
+    const long total = nb * (E / eps) * C.cols;
+    if (total > 0) {
+        const long blocks = std::min(cdiv(total, 256), 148L * 64);
+        k_block_within_subject_norm<<<(unsigned)blocks, 256, 0, st>>>(Z, nb, E, C.cols, C.stride_i, C.ld, C.chunk_step,
+                                                                      C.t256, eps);
+        LAUNCH_CHECK("k_block_within_subject_norm");
+    }
+    const int nt = (E + FGT - 1) / FGT;
+    const long grid = nb * (nt * (nt + 1) / 2);
+    if (grid > 0x7fffffffL) return fail(FCMA_EINVAL, "internal: k_feature_gram_tiled: too many rows in one pass");
+    constexpr size_t smem = 2 * (size_t)NG_CH * FG_LDT * sizeof(double);
+    int rc = kind == 0
+                 ? launch_kernel(k_feature_gram_tiled<0>, (unsigned)grid, NG_THREADS, smem, st, "k_feature_gram_tiled",
+                                 (const float *)Z, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256, K_fit, K_pred)
+                 : launch_kernel(k_feature_gram_tiled<1>, (unsigned)grid, NG_THREADS, smem, st, "k_feature_gram_tiled",
+                                 (const float *)Z, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256, K_fit, K_pred);
+    if (rc || kind == 0) return rc;
+    k_feature_rbf_epilogue<<<(unsigned)nb, 256, 0, st>>>(E, gamma, K_fit, K_pred);
+    LAUNCH_CHECK("k_feature_rbf_epilogue");
+    return FCMA_OK;
+}
+
+// the checks of both feature entry points (who: the entry point the messages name; 1 <= E <= e_max)
+static int voxel_feature_kernels(const char *who, int e_max, bool tiled, const void *rows_op, const void *cols_op,
+                                 int precision, int E, int T, long V, long V2, long start, long nb, int eps, int kind,
+                                 double gamma, float *work_dev, size_t work_bytes, double *K_fit_dev, double *K_pred_dev,
+                                 void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (eps <= 0) return fail(FCMA_EINVAL, "%s: epochs_per_subj must be positive", who);
+    if (E < 1 || E > e_max) return fail(FCMA_EINVAL, "%s: E = %d outside 1..%d", who, E, e_max);
+    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "%s: kind must be 0 (linear) or 1 (rbf)", who);
+    if (!K_fit_dev || (kind == 1 && !K_pred_dev)) return fail(FCMA_EINVAL, "%s: null output", who);
+    if (kind == 1 && !(gamma >= 0.0 && gamma <= 1.7976931348623157e308))
+        return fail(FCMA_EINVAL, "%s: gamma must be finite and non-negative", who);
+    FeatureStage fs{kind, gamma, K_fit_dev, K_pred_dev, tiled};
+    return run_pipeline(rows_op, cols_op, precision, E, T, V, V2, start, nb, eps, 0, work_dev, work_bytes, nullptr, 0,
+                        (cudaStream_t)stream, &fs);
+}
+
 extern "C" int fcma_voxel_feature_kernels(const void *rows_op, const void *cols_op, int precision, int E, int T, long V,
                                           long V2, long start, long nb, int eps, int kind, double gamma, float *work_dev,
                                           size_t work_bytes, double *K_fit_dev, double *K_pred_dev, void *stream)
 {
-    int rc = check_device();
-    if (rc) return rc;
-    if (eps <= 0) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: epochs_per_subj must be positive");
-    if (E < 1 || E > 64) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: E = %d outside 1..64", E);
-    if (kind != 0 && kind != 1) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: kind must be 0 (linear) or 1 (rbf)");
-    if (!K_fit_dev || (kind == 1 && !K_pred_dev)) return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: null output");
-    if (kind == 1 && !(gamma >= 0.0 && gamma <= 1.7976931348623157e308))
-        return fail(FCMA_EINVAL, "fcma_voxel_feature_kernels: gamma must be finite and non-negative");
-    FeatureStage fs{kind, gamma, K_fit_dev, K_pred_dev};
-    return run_pipeline(rows_op, cols_op, precision, E, T, V, V2, start, nb, eps, 0, work_dev, work_bytes, nullptr, 0,
-                        (cudaStream_t)stream, &fs);
+    return voxel_feature_kernels("fcma_voxel_feature_kernels", 64, false, rows_op, cols_op, precision, E, T, V, V2, start,
+                                 nb, eps, kind, gamma, work_dev, work_bytes, K_fit_dev, K_pred_dev, stream);
+}
+
+extern "C" int fcma_voxel_feature_kernels_wide(const void *rows_op, const void *cols_op, int precision, int E, int T,
+                                               long V, long V2, long start, long nb, int eps, int kind, double gamma,
+                                               float *work_dev, size_t work_bytes, double *K_fit_dev, double *K_pred_dev,
+                                               void *stream)
+{
+    return voxel_feature_kernels("fcma_voxel_feature_kernels_wide", 256, true, rows_op, cols_op, precision, E, T, V, V2,
+                                 start, nb, eps, kind, gamma, work_dev, work_bytes, K_fit_dev, K_pred_dev, stream);
 }
 
 // ---------------------------------------------------------------- host-buffer entry points

@@ -311,11 +311,33 @@ def voxel_kernels(rows, cols, start, nb, eps, flags=0, work=None, out=None):
 
 def feature_kernels_f64(rows, cols, start, nb, eps, kind="linear", gamma=None, work=None):
     """a4 -> a6 -> fp64 kernel matrices of the normalised correlation vectors for voxel rows [start, start+nb)
-    (fcma_voxel_feature_kernels): z[i] is the ``[E, V2]`` block ``within_subject_norm_`` gives on the raw correlations,
-    bit for bit.  ``kind='linear'``: returns ``(G, G)``, ``G_ab = sum_j z_aj z_bj``; ``kind='rbf'`` with a number
-    ``gamma``: ``(K_fit, K_pred)``, the x_square form libsvm trains with and the difference form of its decisions.  Both
-    float64 CUDA ``[nb, E, E]``, ready for ``svm_cv_f64``; the result is that of ``SVC(kernel=kind)`` on the features."""
-    lib = _lib.load()
+    (fcma_voxel_feature_kernels, 1 <= E <= 64): z[i] is the ``[E, V2]`` block ``within_subject_norm_`` gives on the raw
+    correlations, bit for bit.  ``kind='linear'``: returns ``(G, G)``, ``G_ab = sum_j z_aj z_bj``; ``kind='rbf'`` with a
+    number ``gamma``: ``(K_fit, K_pred)``, the x_square form libsvm trains with and the difference form of its decisions.
+    Both float64 CUDA ``[nb, E, E]``, ready for ``svm_cv_f64``; the result is that of ``SVC(kernel=kind)`` on the
+    features."""
+    return _feature_kernels(_lib.load().fcma_voxel_feature_kernels, rows, cols, start, nb, eps, kind, gamma, work)
+
+
+def feature_kernels_f64_wide(rows, cols, start, nb, eps, kind="linear", gamma=None, work=None):
+    """``feature_kernels_f64`` for 1 <= E <= 256 (fcma_voxel_feature_kernels_wide: the block normalised in place, then
+    k_feature_gram_tiled): the same arguments and outputs.  D, and so the rbf ``K_pred``, equals ``feature_kernels_f64``'s
+    bit for bit at E <= 64; G is summed in another order of its 4-column MMA steps."""
+    return _feature_kernels(_lib.load().fcma_voxel_feature_kernels_wide, rows, cols, start, nb, eps, kind, gamma, work)
+
+
+def feature_block_rows(E, per_row, n, budget):
+    """Voxel rows per ``feature_kernels_f64_wide`` call: the workspace (``per_row`` bytes a row,
+    ``fcma_work_bytes_per_row``) and the fp64 ``K_fit`` and ``K_pred`` (16 E^2 bytes a row) of at most ``n`` rows within
+    ``budget`` bytes, whole 256-row GEMM blocks when there are more than 256; at least one row."""
+    rows = max(1, min(n, budget // (per_row + 16 * E * E)))
+    if rows >= 256:
+        rows = (rows // 256) * 256
+    return rows
+
+
+def _feature_kernels(entry, rows, cols, start, nb, eps, kind, gamma, work):
+    """The body of feature_kernels_f64 and feature_kernels_f64_wide around one call of the C entry point ``entry``."""
     _check_pair(rows, cols)
     E, V2 = rows.E, cols.V
     if kind not in ("linear", "rbf"):
@@ -333,10 +355,9 @@ def feature_kernels_f64(rows, cols, start, nb, eps, kind="linear", gamma=None, w
     K_fit = torch.empty((nb, E, E), dtype=torch.float64, device=rows.device)
     K_pred = K_fit if kcode == 0 else torch.empty_like(K_fit)
     with torch.cuda.device(rows.device):
-        _lib.check(lib.fcma_voxel_feature_kernels(_ptr(rows.buf), _ptr(cols.buf), _prec_code(rows.precision), E, rows.T,
-                                                  rows.V, V2, start, nb, int(eps), kcode, g, _ptr(work.buf),
-                                                  work.buf.numel(), _ptr(K_fit), _ptr(K_pred) if kcode else None,
-                                                  _stream_ptr()))
+        _lib.check(entry(_ptr(rows.buf), _ptr(cols.buf), _prec_code(rows.precision), E, rows.T, rows.V, V2, start, nb,
+                         int(eps), kcode, g, _ptr(work.buf), work.buf.numel(), _ptr(K_fit),
+                         _ptr(K_pred) if kcode else None, _stream_ptr()))
     return K_fit, K_pred
 
 

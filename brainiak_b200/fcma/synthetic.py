@@ -55,3 +55,21 @@ def make_two_masks(V, V2, T, E, seed=SEED):
     d1, labels = make_epochs(V, T, E, seed=seed)
     d2, _ = make_epochs(V2, T, E, seed=seed + 7919)
     return d1, d2, labels
+
+
+def make_dyadic_epochs(V, T, E, seed=SEED, informative=None):
+    """Like ``make_epochs`` (planted common time course in the first ``informative`` voxels of odd-labelled epochs), but
+    every value is a multiple of 1/32 with magnitude at most 5/32 and ``T <= 40``: every product and every partial sum of
+    a correlation is exact in fp32, so any summation order gives the same r, bit for bit (|r| < 1).  Not normalised."""
+    if T > 40:
+        raise ValueError("T must be at most 40 for exact correlations")
+    if informative is None:
+        informative = max(1, V // 6)
+    data = []
+    for e in range(E):
+        rng = np.random.RandomState(seed + e)
+        m = rng.randint(-3, 4, size=(T, V))
+        if e % 2 == 1:
+            m[:, :informative] += rng.randint(-2, 3, size=(T, 1))
+        data.append(np.ascontiguousarray(m.astype(np.float32) / np.float32(32)))
+    return data, make_labels(E)

@@ -97,8 +97,9 @@ class VoxelSelector:
         two conditions one-vs-one with libsvm's vote, see engine.svm_cv_precomputed) for
         ``SVC(kernel='precomputed')`` on the kernel matrices (at most 256 epochs and 64 folds), and for ``SVC(kernel='linear')`` or ``SVC(kernel='rbf')``
         with ``gamma='auto'`` or a number on the normalised correlation vectors themselves: their fp64 kernel matrices
-        are built on the GPU (engine.feature_kernels_f64, without the decimal shrink, as scikit-learn sees the features)
-        and cross-validated by engine.svm_cv_f64 (at most 64 epochs and folds, no class weights, probability or tie
+        are built on the GPU (engine.feature_kernels_f64, above 64 epochs engine.feature_kernels_f64_wide, without the
+        decimal shrink, as scikit-learn sees the features) and cross-validated by engine.svm_cv_f64 (at most 256 epochs
+        and 64 folds, no class weights, probability or tie
         breaking, and ``mask_self=False``, see engine.svc_feature_kind).  ``False`` or any other classifier ->
         scikit-learn on the host, exactly as the reference (voxelselector.py:41-53)
     """
@@ -343,24 +344,31 @@ class VoxelSelector:
             results += self._cv_block(K[s - k0:s - k0 + nb], s, nb, clf, on_gpu, folds)
         return results
 
-    def _plain_block(self, n):
-        """Rows per pass of the plain (row-block) pipeline, with its scratch allocated for them."""
+    def _plain_block(self, n, fp64_outputs=False):
+        """Rows per pass of the plain (row-block) pipeline, with its scratch allocated for them.  ``fp64_outputs``: the
+        pass also holds the rows' fp64 K_fit and K_pred (engine.feature_block_rows)."""
+        import torch
         rows_op, _ = self._operands()
         E = rows_op.E
-        block = self.block_rows or engine.Workspace.rows_for(E, self.num_voxels2, n, rows_op.device)
+        if self.block_rows or not fp64_outputs:
+            block = self.block_rows or engine.Workspace.rows_for(E, self.num_voxels2, n, rows_op.device)
+        else:
+            free, _ = torch.cuda.mem_get_info(rows_op.device)
+            block = engine.feature_block_rows(E, _lib.load().fcma_work_bytes_per_row(E, self.num_voxels2), n,
+                                              min(free // 2, 32 << 30))
         block = max(1, min(block, n))
         if self._work is None or self._work.rows < block or isinstance(self._work, engine.SymWorkspace):
             self._work = None
             self._work = engine.Workspace(E, self.num_voxels2, block, rows_op.device)
         return block
 
-    def _feature_kind(self, clf):
+    def _feature_kind(self, clf, max_epochs=64):
         """'linear' / 'rbf' when ``clf`` on the normalised correlation vectors is cross-validated on the GPU (fp64 kernel
-        matrices + the fp64 solver), else None.  mask_self is not applied to the features by the host path, so that
-        combination stays there."""
+        matrices + the fp64 solver) at up to ``max_epochs`` epochs, else None.  mask_self is not applied to the features
+        by the host path, so that combination stays there."""
         if not self.gpu_cv or self.mask_self:
             return None
-        return engine.svc_feature_kind(clf, self.labels, self.num_folds, len(self.raw_data))
+        return engine.svc_feature_kind(clf, self.labels, self.num_folds, len(self.raw_data), max_epochs=max_epochs)
 
     def _score_rows(self, start, n, clf):
         """GPU stages for rows [start, start+n) in HBM-sized blocks, then the cross validation (GPU or host)."""
@@ -370,17 +378,19 @@ class VoxelSelector:
         results = []
         if _is_precomputed_svc(clf) and self._symmetric_ok():
             return self._score_rows_symmetric(start, n, clf)
-        kind = None if _is_precomputed_svc(clf) else self._feature_kind(clf)
+        kind = None if _is_precomputed_svc(clf) else self._feature_kind(clf, max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
         if kind is not None:
             # SVC(kernel='linear' | 'rbf') on the features: the fp64 kernels of the features give libsvm's iterations and
             # decisions (DESIGN.md §3.8); gamma='auto' is scikit-learn's 1 / n_features
             gamma = None if kind == 'linear' else (1.0 / self.num_voxels2 if clf.gamma == 'auto' else float(clf.gamma))
-            folds = engine.make_svm_folds(self.labels, self.num_folds)
-            block = self._plain_block(n)
+            wide = E > 64
+            folds = engine.svm_folds_for(self.labels, self.num_folds, E)
+            feature_kernels = engine.feature_kernels_f64_wide if wide else engine.feature_kernels_f64
+            block = self._plain_block(n, fp64_outputs=wide)
             for s in range(start, start + n, block):
                 nb = min(block, start + n - s)
-                K_fit, K_pred = engine.feature_kernels_f64(rows_op, cols_op, s, nb, self.epochs_per_subj, kind, gamma,
-                                                           work=self._work)
+                K_fit, K_pred = feature_kernels(rows_op, cols_op, s, nb, self.epochs_per_subj, kind, gamma,
+                                                work=self._work)
                 acc = engine.svm_cv_f64(K_fit, K_pred, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
                                         max_iter=clf.max_iter, shrinking=bool(clf.shrinking), folds=folds)
                 del K_fit, K_pred

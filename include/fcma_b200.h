@@ -269,6 +269,14 @@ int fcma_searchlight_kernels_wide(const float *vol_dev, long nx, long ny, long n
 int fcma_voxel_feature_kernels(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2,
                                long start, long nb, int eps, int kind, double gamma, float *work_dev, size_t work_bytes,
                                double *K_fit_dev, double *K_pred_dev, void *stream);
+/* The same for 1 <= E <= 256, same arguments and outputs: the raw block is normalised in place (within-subject z, the
+ * same z as above), then one CTA per (row, upper 64 x 64 epoch tile) sums G on the fp64 tensor cores and, for rbf, D on
+ * the FP64 pipe; a per-row epilogue applies the rbf forms.  D (so the rbf K_pred) is bit-identical to
+ * fcma_voxel_feature_kernels' at E <= 64, G is summed in another order of its 4-column steps, every entry in the same
+ * order whichever tile computes it.  Both matrices are exactly symmetric. */
+int fcma_voxel_feature_kernels_wide(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2,
+                                    long start, long nb, int eps, int kind, double gamma, float *work_dev,
+                                    size_t work_bytes, double *K_fit_dev, double *K_pred_dev, void *stream);
 
 /* ---- a12 / a15: plain NT GEMM  C[m][n] = sum_k A[m][k]*B[n][k]  (fp32 FFMA, row-major) ---------- */
 int fcma_gemm_nt(const float *A_dev, const float *B_dev, float *C_dev, long M, long N, long K,
