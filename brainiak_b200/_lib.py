@@ -86,6 +86,14 @@ SIGNATURES = {
     "fcma_voxel_feature_kernels_wide": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_long, c_long, c_long, c_long,
                                                 c_int, c_int, ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p,
                                                 c_void_p]),
+    "fcma_voxel_feature_gram_wide": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_long, c_long, c_long, c_long,
+                                             c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_searchlight_gram_wide": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                           c_long, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fcma_fold_gammas": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, c_void_p, c_long, c_void_p, c_void_p,
+                                 c_void_p]),
+    "fcma_rbf_fold_kernels": (c_int, [c_void_p, c_void_p, c_long, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p]),
     "fcma_gemm_nt": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_long, c_long, c_long, c_long,
                              c_long, c_void_p]),
     "fcma_row_normalize": (c_int, [c_void_p, c_long, c_long, c_long, c_int, c_void_p]),

@@ -3046,17 +3046,19 @@ static bool half_block(int precision, int flags)
 
 // Second stage of fcma_voxel_feature_kernels (E <= 64: k_norm_gram_f64) and fcma_voxel_feature_kernels_wide (tiled:
 // E <= 256): the per-voxel fp64 kernel matrices of the normalised correlation vectors instead of the fp32 SYRK.  kind 0
-// linear, 1 rbf; outputs [nb][E][E].
+// linear, 1 rbf, 2 G and D as they are (tiled only); outputs [nb][E][E].  moments (tiled only, may be null): the
+// per-sample sums of the normalised block, [nb][E][4] doubles (k_block_moments).
 struct FeatureStage {
     int kind;
     double gamma;
     double *K_fit, *K_pred;
     bool tiled;
+    double *moments = nullptr;
 };
 static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
                                 cudaStream_t st);
 static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
-                                     cudaStream_t st);
+                                     double *moments, cudaStream_t st);
 
 // shared body of the fused pipelines; with `feat` the GEMM writes raw r and the feature stage replaces normalise+SYRK
 static int run_pipeline(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2, long start,
@@ -3099,8 +3101,10 @@ static int run_pipeline(const void *rows_op, const void *cols_op, int precision,
         const float beta = sum_over_rows ? 1.0f : 0.0f;
         if (feat) {
             const size_t off = (size_t)done * E * E;
-            rc = (feat->tiled ? launch_feature_gram_tiled : launch_norm_gram_f64)(
-                C, eps, feat->kind, feat->gamma, feat->K_fit + off, feat->K_pred ? feat->K_pred + off : nullptr, st);
+            double *K_pred = feat->K_pred ? feat->K_pred + off : nullptr;
+            rc = feat->tiled ? launch_feature_gram_tiled(C, eps, feat->kind, feat->gamma, feat->K_fit + off, K_pred,
+                                                         feat->moments ? feat->moments + (size_t)done * E * 4 : nullptr, st)
+                             : launch_norm_gram_f64(C, eps, feat->kind, feat->gamma, feat->K_fit + off, K_pred, st);
         } else if (tiled || (normalise && fused)) {
             rc = launch_norm_syrk(C, normalise ? eps : 0, (normalise && fisher_in_gemm) ? 1 : 0,
                                   mask_self ? start + done : -1, beta, Kdst, sum_over_rows, st);
@@ -4197,6 +4201,45 @@ __device__ __forceinline__ double rbf_fit(double gamma, double gaa, double gbb, 
 }
 __device__ __forceinline__ double rbf_pred(double gamma, double d) { return exp(__dmul_rn(-gamma, d)); }
 
+// Double-double arithmetic (hi + lo, |lo| <= ulp(hi) / 2) for the per-sample moments of SVC(gamma='scale') and the fold
+// variances built from them.  Every operation is rounded separately, so a sum taken in a fixed order is bit-reproducible.
+struct DD {
+    double hi, lo;
+};
+__device__ __forceinline__ DD dd_fast_two_sum(double a, double b)   // |a| >= |b| or a == 0
+{
+    const double s = __dadd_rn(a, b);
+    return {s, __dsub_rn(b, __dsub_rn(s, a))};
+}
+__device__ __forceinline__ DD dd_two_sum(double a, double b)
+{
+    const double s = __dadd_rn(a, b), bp = __dsub_rn(s, a);
+    return {s, __dadd_rn(__dsub_rn(a, __dsub_rn(s, bp)), __dsub_rn(b, bp))};
+}
+__device__ __forceinline__ DD dd_add(DD a, DD b)
+{
+    const DD s = dd_two_sum(a.hi, b.hi), t = dd_two_sum(a.lo, b.lo);
+    const DD u = dd_fast_two_sum(s.hi, __dadd_rn(s.lo, t.hi));
+    return dd_fast_two_sum(u.hi, __dadd_rn(u.lo, t.lo));
+}
+__device__ __forceinline__ DD dd_add_d(DD a, double x)
+{
+    const DD s = dd_two_sum(a.hi, x);
+    return dd_fast_two_sum(s.hi, __dadd_rn(s.lo, a.lo));
+}
+__device__ __forceinline__ DD dd_mul(DD a, DD b)
+{
+    const double p = __dmul_rn(a.hi, b.hi), e = __fma_rn(a.hi, b.hi, -p);
+    return dd_fast_two_sum(p, __dadd_rn(e, __dadd_rn(__dmul_rn(a.hi, b.lo), __dmul_rn(a.lo, b.hi))));
+}
+__device__ __forceinline__ DD dd_div_d(DD a, double b)
+{
+    const double q1 = __ddiv_rn(a.hi, b), p = __dmul_rn(q1, b), pe = __fma_rn(q1, b, -p);
+    const DD r = dd_two_sum(a.hi, -p);
+    const double q2 = __ddiv_rn(__dadd_rn(__dsub_rn(r.lo, pe), __dadd_rn(r.hi, a.lo)), b);
+    return dd_fast_two_sum(q1, q2);
+}
+
 template <int KIND>
 __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float *__restrict__ vol, int ny, int nz, int E,
                                                                     const unsigned char *__restrict__ mask, int r,
@@ -4307,7 +4350,8 @@ __global__ void __launch_bounds__(SL_THREADS) k_searchlight_kernels(const float 
 // depends on x_a and x_b only, never on E or on the tile.  rbf: threads 0..SLT-1 sum G_aa of the row epochs and threads
 // SLT..2 SLT-1 G_bb of the column epochs in the same order.  The tile goes out through shared memory in coalesced rows;
 // an off-diagonal tile also as its mirror image (J, I), and a diagonal tile stores its entries a <= b at (a, b) and
-// (b, a), so both matrices are exactly symmetric.
+// (b, a), so both matrices are exactly symmetric.  KIND 2 (SVC(gamma='scale'), whose gamma is known per fold only):
+// K_fit = G and K_pred = D = sum_f (x_a - x_b)^2 as summed for rbf, not exponentiated.
 #define SLT 64
 #define SLT_PITCH 65   // doubles per staged tile row: the mirror's column reads hit distinct bank pairs
 
@@ -4371,7 +4415,7 @@ __global__ void __launch_bounds__(SL_THREADS, 2)
 #pragma unroll
                 for (int v = 0; v < 4; v++) {
                     g[u][v] = __dadd_rn(g[u][v], __dmul_rn(xa[u], xb[v]));
-                    if (KIND == 1) {
+                    if (KIND != 0) {
                         const double df = __dsub_rn(xa[u], xb[v]);
                         d[u][v] = __dadd_rn(d[u][v], __dmul_rn(df, df));
                     }
@@ -4387,7 +4431,7 @@ __global__ void __launch_bounds__(SL_THREADS, 2)
     const double gm = KIND == 1 ? gamma[m] : 0.0;
     double *const out[2] = {K_fit + (size_t)m * E * E, K_pred + (size_t)m * E * E};
 #pragma unroll
-    for (int pass = 0; pass < (KIND == 1 ? 2 : 1); pass++) {
+    for (int pass = 0; pass < (KIND != 0 ? 2 : 1); pass++) {
         __syncthreads();      // the staged features (pass 0) or the previous tile (pass 1) are no longer read
 #pragma unroll
         for (int u = 0; u < 4; u++)
@@ -4397,6 +4441,7 @@ __global__ void __launch_bounds__(SL_THREADS, 2)
                 if (a >= nr || b >= nc || (I == J && a > b)) continue;
                 double val = g[u][v];
                 if (KIND == 1) val = pass == 0 ? rbf_fit(gm, s_diag[0][a], s_diag[1][b], g[u][v]) : rbf_pred(gm, d[u][v]);
+                if (KIND == 2 && pass == 1) val = d[u][v];
                 s_tile[a * SLT_PITCH + b] = val;
                 if (I == J) s_tile[b * SLT_PITCH + a] = val;
             }
@@ -4487,6 +4532,56 @@ extern "C" int fcma_searchlight_kernels_wide(const float *vol_dev, long nx, long
                              K_fit_dev);
     return launch_kernel(k_searchlight_kernels_tiled<1>, grid, SL_THREADS, 0, st, "k_searchlight_kernels_tiled", vol_dev,
                          (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, gdev, K_fit_dev, K_pred_dev);
+}
+
+// Per-sample moments of the searchlight features: thread (centre m, epoch e) sums s = sum_f x_e[f] and q = sum_f x_e[f]^2
+// over the centre's features in cube order, in double-double (x^2 of a float is exact in double).  moments[(m E + e) 4 +
+// 0..3] = s.hi, s.lo, q.hi, q.lo.
+__global__ void __launch_bounds__(256) k_searchlight_moments(const float *__restrict__ vol, int ny, int nz, int E,
+                                                             const unsigned char *__restrict__ mask, int r,
+                                                             const unsigned char *__restrict__ shape,
+                                                             const long *__restrict__ centres, long M,
+                                                             double *__restrict__ moments)
+{
+    const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= M * E) return;
+    const long m = idx / E;
+    const int e = (int)(idx - m * E);
+    const long c = centres[m];
+    const int cz = (int)(c % nz), cy = (int)((c / nz) % ny), cx = (int)(c / ((long)nz * ny));
+    const int side = 2 * r + 1, ncube = side * side * side;
+    DD s{0.0, 0.0}, q{0.0, 0.0};
+    for (int o = 0; o < ncube; o++) {
+        const int i = o / (side * side), j = (o / side) % side, k = o % side;
+        const long vox = ((long)(cx - r + i) * ny + (cy - r + j)) * nz + (cz - r + k);
+        if (!(shape[o] && mask[vox])) continue;
+        const double x = (double)vol[vox * E + e];
+        s = dd_add_d(s, x);
+        q = dd_add_d(q, __dmul_rn(x, x));
+    }
+    double *out = moments + idx * 4;
+    out[0] = s.hi, out[1] = s.lo, out[2] = q.hi, out[3] = q.lo;
+}
+
+extern "C" int fcma_searchlight_gram_wide(const float *vol_dev, long nx, long ny, long nz, int E,
+                                          const unsigned char *mask_dev, int sl_rad, const unsigned char *shape_dev,
+                                          const long *centres_host, long M, double *G_dev, double *D_dev,
+                                          double *moments_dev, void *stream)
+{
+    cudaStream_t st = (cudaStream_t)stream;
+    AsyncBuf cbuf, gbuf;
+    if (!D_dev || !moments_dev) return fail(FCMA_EINVAL, "fcma_searchlight_gram_wide: null output");
+    int rc = searchlight_args("fcma_searchlight_gram_wide", 256, vol_dev, nx, ny, nz, E, mask_dev, sl_rad, shape_dev,
+                              centres_host, M, 0, nullptr, G_dev, D_dev, st, cbuf, gbuf);
+    if (rc) return rc;
+    const int nt = (E + SLT - 1) / SLT;
+    const dim3 grid((unsigned)M, nt * (nt + 1) / 2);
+    const long *cdev = static_cast<const long *>(cbuf.p);
+    rc = launch_kernel(k_searchlight_kernels_tiled<2>, grid, SL_THREADS, 0, st, "k_searchlight_kernels_tiled", vol_dev,
+                       (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, (const double *)nullptr, G_dev, D_dev);
+    if (rc) return rc;
+    return launch_kernel(k_searchlight_moments, (unsigned)cdiv(M * E, 256), 256, 0, st, "k_searchlight_moments", vol_dev,
+                         (int)ny, (int)nz, E, mask_dev, sl_rad, shape_dev, cdev, M, moments_dev);
 }
 
 // ============================================================================================
@@ -4697,6 +4792,8 @@ static int launch_norm_gram_f64(const CorrBlock &C, int eps, int kind, double ga
 //                                both matrices are exactly symmetric.  rbf: K_fit holds G and K_pred holds D.
 //   k_feature_rbf_epilogue       rbf: K_fit = rbf_fit(G_aa, G_bb, G_ab), K_pred = rbf_pred(D) in place, per row (G_aa
 //                                comes from other CTAs' diagonal tiles).  K_fit_aa = K_pred_aa = 1 exactly.
+// kind 2 (SVC(gamma='scale'), whose gamma is known per fold only) runs k_feature_gram_tiled<1> without the epilogue, and
+// k_block_moments after the normalisation writes the per-sample sums s_a = sum_j z_aj and q_a = sum_j z_aj^2.
 // No atomics: two runs are bit-identical.
 #define FGT 64
 #define FG_LDT (FGT + 4)     // doubles per staged column: conflict-free widening, MMA fragments and D reads
@@ -4717,6 +4814,38 @@ __global__ void __launch_bounds__(256) k_block_within_subject_norm(float *C, lon
         const long j = idx % n2, v = idx / n2, s = v % nsubj, i = v / nsubj;
         within_subject_column(C + block_row_off(i, stride_i, chunk_step, t256) + (j / 256) * chunk_step + j % 256, ld, s,
                               eps);
+    }
+}
+
+// Per-sample moments of the normalised block: warp (row i, epoch e) sums s = sum_j z_ej and q = sum_j z_ej^2 in
+// double-double, lane l over the columns j = l (mod 32) in order, then the lanes in a fixed butterfly.  moments[(i E + e) 4
+// + 0..3] = s.hi, s.lo, q.hi, q.lo.
+__global__ void __launch_bounds__(256) k_block_moments(const float *__restrict__ Z, long nb, int E, long n2, long stride_i,
+                                                       long ld, long chunk_step, long t256, double *__restrict__ moments)
+{
+    const int lane = threadIdx.x & 31;
+    const long nwarps = (long)gridDim.x * (blockDim.x >> 5);
+    for (long w = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < nb * E; w += nwarps) {
+        const long i = w / E;
+        const int e = (int)(w - i * E);
+        const float *Zi = Z + block_row_off(i, stride_i, chunk_step, t256) + (long)e * ld;
+        DD s{0.0, 0.0}, q{0.0, 0.0};
+        for (long j = lane; j < n2; j += 32) {
+            const double x = (double)Zi[(j / 256) * chunk_step + j % 256];
+            s = dd_add_d(s, x);
+            q = dd_add_d(q, __dmul_rn(x, x));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const DD s2{__shfl_xor_sync(0xffffffffu, s.hi, o), __shfl_xor_sync(0xffffffffu, s.lo, o)};
+            const DD q2{__shfl_xor_sync(0xffffffffu, q.hi, o), __shfl_xor_sync(0xffffffffu, q.lo, o)};
+            s = dd_add(s, s2);
+            q = dd_add(q, q2);
+        }
+        if (lane == 0) {
+            double *out = moments + w * 4;
+            out[0] = s.hi, out[1] = s.lo, out[2] = q.hi, out[3] = q.lo;
+        }
     }
 }
 
@@ -4875,7 +5004,7 @@ __global__ void __launch_bounds__(256) k_feature_rbf_epilogue(int E, double gamm
 
 // over the raw fp32 correlation block C, tiled or strided; normalises C in place
 static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, double gamma, double *K_fit, double *K_pred,
-                                     cudaStream_t st)
+                                     double *moments, cudaStream_t st)
 {
     const int E = C.E;
     const long nb = C.rows;
@@ -4889,6 +5018,12 @@ static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, doub
                                                                       C.t256, eps);
         LAUNCH_CHECK("k_block_within_subject_norm");
     }
+    if (moments) {
+        const long blocks = std::min(cdiv(nb * E, 8), 148L * 64);
+        k_block_moments<<<(unsigned)blocks, 256, 0, st>>>(Z, nb, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256,
+                                                          moments);
+        LAUNCH_CHECK("k_block_moments");
+    }
     const int nt = (E + FGT - 1) / FGT;
     const long grid = nb * (nt * (nt + 1) / 2);
     if (grid > 0x7fffffffL) return fail(FCMA_EINVAL, "internal: k_feature_gram_tiled: too many rows in one pass");
@@ -4898,7 +5033,7 @@ static int launch_feature_gram_tiled(const CorrBlock &C, int eps, int kind, doub
                                  (const float *)Z, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256, K_fit, K_pred)
                  : launch_kernel(k_feature_gram_tiled<1>, (unsigned)grid, NG_THREADS, smem, st, "k_feature_gram_tiled",
                                  (const float *)Z, E, C.cols, C.stride_i, C.ld, C.chunk_step, C.t256, K_fit, K_pred);
-    if (rc || kind == 0) return rc;
+    if (rc || kind != 1) return rc;
     k_feature_rbf_epilogue<<<(unsigned)nb, 256, 0, st>>>(E, gamma, K_fit, K_pred);
     LAUNCH_CHECK("k_feature_rbf_epilogue");
     return FCMA_OK;
@@ -4938,6 +5073,109 @@ extern "C" int fcma_voxel_feature_kernels_wide(const void *rows_op, const void *
 {
     return voxel_feature_kernels("fcma_voxel_feature_kernels_wide", 256, true, rows_op, cols_op, precision, E, T, V, V2,
                                  start, nb, eps, kind, gamma, work_dev, work_bytes, K_fit_dev, K_pred_dev, stream);
+}
+
+extern "C" int fcma_voxel_feature_gram_wide(const void *rows_op, const void *cols_op, int precision, int E, int T, long V,
+                                            long V2, long start, long nb, int eps, float *work_dev, size_t work_bytes,
+                                            double *G_dev, double *D_dev, double *moments_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (eps <= 0) return fail(FCMA_EINVAL, "fcma_voxel_feature_gram_wide: epochs_per_subj must be positive");
+    if (E < 1 || E > 256) return fail(FCMA_EINVAL, "fcma_voxel_feature_gram_wide: E = %d outside 1..256", E);
+    if (!G_dev || !D_dev || !moments_dev) return fail(FCMA_EINVAL, "fcma_voxel_feature_gram_wide: null output");
+    FeatureStage fs{2, 0.0, G_dev, D_dev, true, moments_dev};
+    return run_pipeline(rows_op, cols_op, precision, E, T, V, V2, start, nb, eps, 0, work_dev, work_bytes, nullptr, 0,
+                        (cudaStream_t)stream, &fs);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// SVC(kernel='rbf', gamma='scale') per fold.  scikit-learn's BaseLibSVM.fit sets gamma = 1 / (F * X.var()) (1 if the
+// variance is 0) on the fold's float64 training matrix X [n_train][F].  k_fold_gammas: thread (item, fold) sums the
+// moments of the fold's training samples in double-double, rounds var = Q / N - (S / N)^2 (N = n_train F) once, and applies
+// scikit-learn's two roundings F * var and 1 / that.  It flags the (item, fold) whose exact variance and NumPy's two-pass
+// variance can differ by more than a few ulps: mean^2 > 2^36 var, which includes var == 0 with a nonzero feature
+// (DESIGN.md §3.9).
+__global__ void __launch_bounds__(256) k_fold_gammas(const double *__restrict__ moments, long n, int E, int nfolds,
+                                                     const unsigned char *__restrict__ train,
+                                                     const long *__restrict__ nfeat_per_item, long nfeat,
+                                                     double *__restrict__ gamma, unsigned char *__restrict__ flag)
+{
+    const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n * nfolds) return;
+    const long item = idx / nfolds;
+    const int f = (int)(idx - item * nfolds);
+    const double *mo = moments + item * E * 4;
+    DD S{0.0, 0.0}, Q{0.0, 0.0};
+    long ntr = 0;
+    for (int a = 0; a < E; a++) {
+        if (!train[f * E + a]) continue;
+        S = dd_add(S, DD{mo[4 * a], mo[4 * a + 1]});
+        Q = dd_add(Q, DD{mo[4 * a + 2], mo[4 * a + 3]});
+        ntr++;
+    }
+    const double F = (double)(nfeat_per_item ? nfeat_per_item[item] : nfeat);
+    const double N = __dmul_rn((double)ntr, F);   // exact: below 2^53
+    const DD mean = dd_div_d(S, N);
+    const DD v = dd_add(dd_div_d(Q, N), dd_mul(DD{-mean.hi, -mean.lo}, mean));
+    const double var = v.hi > 0.0 ? v.hi : 0.0;   // v.hi = fl(exact variance) up to ~2^-100 mean^2
+    gamma[idx] = var != 0.0 ? __ddiv_rn(1.0, __dmul_rn(F, var)) : 1.0;
+    flag[idx] = __dmul_rn(mean.hi, mean.hi) > __dmul_rn(0x1p36, var) ? 1 : 0;
+}
+
+// K_fit = rbf_fit(gamma, G_aa, G_bb, G_ab), K_pred = rbf_pred(gamma, D) of one fold, out of place: block per item, its
+// gamma gamma[item * nfolds + fold].  The same operations as k_feature_rbf_epilogue, so the same bits for the same gamma.
+__global__ void __launch_bounds__(256) k_rbf_fold_kernels(const double *__restrict__ G, const double *__restrict__ D,
+                                                          int E, const double *__restrict__ gamma, int nfolds, int fold,
+                                                          double *__restrict__ K_fit, double *__restrict__ K_pred)
+{
+    __shared__ double s_diag[256];
+    const size_t base = (size_t)blockIdx.x * E * E;
+    const double g = gamma[(size_t)blockIdx.x * nfolds + fold];
+    for (int a = threadIdx.x; a < E; a += blockDim.x) s_diag[a] = G[base + (size_t)a * E + a];
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < E * E; idx += blockDim.x) {
+        const int a = idx / E, b = idx - a * E;
+        K_fit[base + idx] = rbf_fit(g, s_diag[a], s_diag[b], G[base + idx]);
+        K_pred[base + idx] = rbf_pred(g, D[base + idx]);
+    }
+}
+
+extern "C" int fcma_fold_gammas(const double *moments_dev, long n, int E, int nfolds, const unsigned char *train_host,
+                                const long *nfeat_dev, long nfeat, double *gamma_dev, unsigned char *flag_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (!moments_dev || !train_host || !gamma_dev || !flag_dev || n <= 0)
+        return fail(FCMA_EINVAL, "fcma_fold_gammas: null buffer or no items");
+    if (E < 1 || E > 256) return fail(FCMA_EINVAL, "fcma_fold_gammas: E = %d outside 1..256", E);
+    if (nfolds < 1 || nfolds > 256) return fail(FCMA_EINVAL, "fcma_fold_gammas: %d folds outside 1..256", nfolds);
+    if (!nfeat_dev && nfeat < 1) return fail(FCMA_EINVAL, "fcma_fold_gammas: no features");
+    for (int f = 0; f < nfolds; f++) {
+        int ntr = 0;
+        for (int a = 0; a < E; a++) ntr += train_host[f * E + a] != 0;
+        if (ntr == 0) return fail(FCMA_EINVAL, "fcma_fold_gammas: fold %d has no training sample", f);
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    AsyncBuf tbuf;
+    CUDA_TRY(tbuf.alloc((size_t)nfolds * E, st));
+    CUDA_TRY(cudaMemcpyAsync(tbuf.p, train_host, (size_t)nfolds * E, cudaMemcpyHostToDevice, st));
+    return launch_kernel(k_fold_gammas, (unsigned)cdiv(n * nfolds, 256), 256, 0, st, "k_fold_gammas", moments_dev, n, E,
+                         nfolds, (const unsigned char *)tbuf.p, nfeat_dev, nfeat, gamma_dev, flag_dev);
+}
+
+extern "C" int fcma_rbf_fold_kernels(const double *G_dev, const double *D_dev, long n, int E, const double *gamma_dev,
+                                     int nfolds, int fold, double *K_fit_dev, double *K_pred_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (!G_dev || !D_dev || !gamma_dev || !K_fit_dev || !K_pred_dev || n <= 0)
+        return fail(FCMA_EINVAL, "fcma_rbf_fold_kernels: null buffer or no items");
+    if (E < 1 || E > 256) return fail(FCMA_EINVAL, "fcma_rbf_fold_kernels: E = %d outside 1..256", E);
+    if (fold < 0 || fold >= nfolds) return fail(FCMA_EINVAL, "fcma_rbf_fold_kernels: fold %d outside 0..%d", fold, nfolds - 1);
+    if (n > 0x7fffffffL) return fail(FCMA_EINVAL, "fcma_rbf_fold_kernels: too many items in one call");
+    return launch_kernel(k_rbf_fold_kernels, (unsigned)n, 256, 0, (cudaStream_t)stream, "k_rbf_fold_kernels", G_dev, D_dev,
+                         E, gamma_dev, nfolds, fold, K_fit_dev, K_pred_dev);
 }
 
 // ---------------------------------------------------------------- host-buffer entry points

@@ -326,14 +326,35 @@ def feature_kernels_f64_wide(rows, cols, start, nb, eps, kind="linear", gamma=No
     return _feature_kernels(_lib.load().fcma_voxel_feature_kernels_wide, rows, cols, start, nb, eps, kind, gamma, work)
 
 
-def feature_block_rows(E, per_row, n, budget):
+def feature_block_rows(E, per_row, n, budget, matrices=2):
     """Voxel rows per ``feature_kernels_f64_wide`` call: the workspace (``per_row`` bytes a row,
     ``fcma_work_bytes_per_row``) and the fp64 ``K_fit`` and ``K_pred`` (16 E^2 bytes a row) of at most ``n`` rows within
-    ``budget`` bytes, whole 256-row GEMM blocks when there are more than 256; at least one row."""
-    rows = max(1, min(n, budget // (per_row + 16 * E * E)))
+    ``budget`` bytes, whole 256-row GEMM blocks when there are more than 256; at least one row.  ``matrices``: the fp64
+    ``[E, E]`` matrices a row holds (4 for ``feature_gram_wide``'s G and D plus one fold's ``K_fit`` and ``K_pred``)."""
+    rows = max(1, min(n, budget // (per_row + 8 * matrices * E * E)))
     if rows >= 256:
         rows = (rows // 256) * 256
     return rows
+
+
+def feature_gram_wide(rows, cols, start, nb, eps, work=None):
+    """The fp64 sums behind ``SVC(kernel='rbf', gamma='scale')`` on the normalised correlation vectors of voxel rows
+    [start, start+nb) (fcma_voxel_feature_gram_wide, 1 <= E <= 256): ``(G, D, moments)``, G and D float64 CUDA
+    ``[nb, E, E]`` -- the entries ``feature_kernels_f64_wide(kind='rbf')`` exponentiates, bit for bit -- and ``moments``
+    float64 ``[nb, E, 4]``: the double-double sums (s.hi, s.lo, q.hi, q.lo) of s_e = sum_j z_ej and q_e = sum_j z_ej^2."""
+    lib = _lib.load()
+    _check_pair(rows, cols)
+    E, V2 = rows.E, cols.V
+    if work is None:
+        work = Workspace(E, V2, Workspace.rows_for(E, V2, nb, rows.device), rows.device)
+    G = torch.empty((nb, E, E), dtype=torch.float64, device=rows.device)
+    D = torch.empty_like(G)
+    moments = torch.empty((nb, E, 4), dtype=torch.float64, device=rows.device)
+    with torch.cuda.device(rows.device):
+        _lib.check(lib.fcma_voxel_feature_gram_wide(_ptr(rows.buf), _ptr(cols.buf), _prec_code(rows.precision), E, rows.T,
+                                                    rows.V, V2, start, nb, int(eps), _ptr(work.buf), work.buf.numel(),
+                                                    _ptr(G), _ptr(D), _ptr(moments), _stream_ptr()))
+    return G, D, moments
 
 
 def _feature_kernels(entry, rows, cols, start, nb, eps, kind, gamma, work):
@@ -683,6 +704,27 @@ def svc_feature_kind(clf, labels, num_folds, E, max_epochs=64):
     return kind
 
 
+def svc_scale_supported(clf, labels, num_folds, E):
+    """True if ``cross_val_score(clf, X, labels, cv=StratifiedKFold(num_folds))`` on float32 features ``X`` (E samples)
+    can be computed by ``svm_cv_scale``: ``SVC(kernel='rbf', gamma='scale')`` -- scikit-learn's ``SVC()`` -- without class
+    weights, probability or tie breaking, E <= ``SVM_WIDE_MAX_EPOCHS``, at most 64 folds that ``svm_folds_for``
+    accepts.  The other rbf gammas and the linear kernel are ``svc_feature_kind``'s."""
+    import sklearn.svm
+    if not (isinstance(clf, sklearn.svm.SVC) and clf.kernel == 'rbf' and isinstance(clf.gamma, str)
+            and clf.gamma == 'scale'):
+        return False
+    # scikit-learn >= 1.9 uses the string 'deprecated' as the default of `probability`
+    if clf.class_weight is not None or getattr(clf, 'probability', False) is True or getattr(clf, 'break_ties', False):
+        return False
+    if E > SVM_WIDE_MAX_EPOCHS or num_folds > 64:
+        return False
+    try:
+        svm_folds_for(labels, num_folds, E)
+    except ValueError:
+        return False
+    return True
+
+
 class SvmFolds:
     """Fold problems for the batched GPU solver: ``structs`` holds one _SvmFold per (fold, class pair) -- pair-major
     inside a fold, pairs in libsvm's order (0,1), (0,2), ..., (1,2), ... -- and everything the vote needs."""
@@ -715,6 +757,25 @@ def svm_folds_for(labels, num_folds, E):
     """The fold problems ``svm_cv_precomputed`` solves E-epoch kernels with: ``make_svm_folds`` up to 64 epochs, else
     ``make_svm_folds_wide``."""
     return make_svm_folds(labels, num_folds) if E <= 64 else make_svm_folds_wide(labels, num_folds)
+
+
+def fold_problems(folds, f):
+    """The problems of fold ``f`` alone: an SvmFolds of one fold whose structs are the slice
+    ``[f * npairs, (f + 1) * npairs)`` of ``folds.structs``, with that fold's ``n_test`` and ``test_labels``."""
+    npairs = len(folds.pairs)
+    struct = folds.structs._type_
+    part = (struct * npairs)(*folds.structs[f * npairs:(f + 1) * npairs])
+    return SvmFolds(part, folds.n_test[f:f + 1], folds.classes, folds.pairs, folds.test_labels[f:f + 1])
+
+
+def fold_train_mask(folds, E):
+    """uint8 ``[num_folds, E]``: 1 where epoch e is a training sample of fold f (every sample outside its held-out part)."""
+    train = np.ones((folds.num_folds, E), dtype=np.uint8)
+    npairs = len(folds.pairs)
+    for f in range(folds.num_folds):
+        fd = folds.structs[f * npairs]
+        train[f, list(fd.test_idx[:fd.n_test])] = 0
+    return train
 
 
 def _build_svm_folds(labels, num_folds, struct, limit):
@@ -783,14 +844,11 @@ def _max_iter_arg(max_iter):
     return -1 if max_iter is None or max_iter < 0 else int(max_iter)
 
 
-def _svm_cv(solve, kernels, K, labels, num_folds, C, tol, max_iter, shrinking, folds, return_iters):
-    """The body of svm_cv_precomputed and svm_cv_f64 around one call of the batched solver ``solve``
-    (fcma_svm_cv_solve or fcma_svm_cv_solve_f64, whose leading arguments are the kernel pointers ``kernels``; ``K`` is
-    one of those kernels): fold problems, outputs, libsvm's one-vs-one vote for more than two classes, and the mean
-    accuracy per kernel."""
+def _svm_correct(solve, kernels, K, C, tol, max_iter, shrinking, folds, return_iters):
+    """One call of the batched solver ``solve`` on the problems of ``folds`` (libsvm's one-vs-one vote for more than two
+    classes): the int32 CUDA ``[nv, num_folds]`` counts of correctly predicted held-out samples, and the ``[nv,
+    nproblems]`` iteration counts (or None)."""
     nv, E, _ = K.shape
-    if folds is None:
-        folds = make_svm_folds(labels, num_folds)
     nprob = folds.nproblems
     two = len(folds.classes) == 2
     with torch.cuda.device(K.device):
@@ -803,6 +861,17 @@ def _svm_cv(solve, kernels, K, labels, num_folds, C, tol, max_iter, shrinking, f
                          _ptr(bits) if not two else None, _ptr(iters) if iters is not None else None, _stream_ptr()))
         if not two:
             correct = _ovo_vote(bits, folds)
+    return correct, iters
+
+
+def _svm_cv(solve, kernels, K, labels, num_folds, C, tol, max_iter, shrinking, folds, return_iters):
+    """The body of svm_cv_precomputed and svm_cv_f64 around one call of the batched solver ``solve``
+    (fcma_svm_cv_solve or fcma_svm_cv_solve_f64, whose leading arguments are the kernel pointers ``kernels``; ``K`` is
+    one of those kernels): fold problems, outputs, libsvm's one-vs-one vote for more than two classes, and the mean
+    accuracy per kernel."""
+    if folds is None:
+        folds = make_svm_folds(labels, num_folds)
+    correct, iters = _svm_correct(solve, kernels, K, C, tol, max_iter, shrinking, folds, return_iters)
     scores = correct.cpu().numpy().astype(np.float64) / folds.n_test[None, :]   # accuracy_score per fold
     acc = scores.mean(axis=1)                                                   # cross_val_score(...).mean()
     return (acc, iters.cpu().numpy()) if return_iters else acc
@@ -844,6 +913,94 @@ def svm_cv_f64(K_fit, K_pred, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, s
     solve = lib.fcma_svm_cv_solve_f64_wide if folds is not None and folds.wide else lib.fcma_svm_cv_solve_f64
     return _svm_cv(solve, (_ptr(K_fit), _ptr(K_pred)), K_fit, labels, num_folds, C, tol, max_iter, shrinking, folds,
                    return_iters)
+
+
+def _check_gd(G, D):
+    if G.dtype != torch.float64 or D.dtype != torch.float64 or G.shape != D.shape or G.dim() != 3 \
+            or G.shape[1] != G.shape[2] or not (G.is_contiguous() and D.is_contiguous()):
+        raise ValueError("G and D must be contiguous float64 [n, E, E] of the same shape")
+
+
+def fold_gammas(moments, train, nfeat):
+    """scikit-learn's ``gamma='scale'`` per (item, fold) from per-sample moments (fcma_fold_gammas): ``moments`` float64
+    CUDA ``[n, E, 4]`` (``feature_gram_wide`` / ``searchlight_gram_wide``), ``train`` uint8 ``[num_folds, E]``
+    (``fold_train_mask``), ``nfeat`` the feature count: a number, or one per item.  Returns ``(gamma, flagged)``: float64
+    and bool CUDA ``[n, num_folds]``; ``flagged`` marks where NumPy's two-pass variance may differ from the exact one by
+    more than a few ulps (DESIGN.md §3.9)."""
+    lib = _lib.load()
+    if moments.dtype != torch.float64 or moments.dim() != 3 or moments.shape[2] != 4 or not moments.is_contiguous():
+        raise ValueError("moments must be contiguous float64 [n, E, 4]")
+    n, E, _ = moments.shape
+    train = np.ascontiguousarray(train, dtype=np.uint8)
+    if train.ndim != 2 or train.shape[1] != E:
+        raise ValueError("train must be [num_folds, %d]" % E)
+    nf = np.asarray(nfeat, dtype=np.int64)
+    if nf.ndim > 1 or (nf.ndim == 1 and len(nf) != n) or (nf < 1).any():
+        raise ValueError("nfeat must be a positive number or one per item (%d)" % n)
+    nfeat_dev = torch.from_numpy(nf).to(moments.device) if nf.ndim == 1 else None
+    nfolds = train.shape[0]
+    gamma = torch.empty((n, nfolds), dtype=torch.float64, device=moments.device)
+    flag = torch.empty((n, nfolds), dtype=torch.uint8, device=moments.device)
+    with torch.cuda.device(moments.device):
+        _lib.check(lib.fcma_fold_gammas(_ptr(moments), n, E, nfolds, train.ctypes.data_as(ctypes.c_void_p),
+                                        _ptr(nfeat_dev) if nfeat_dev is not None else None,
+                                        int(nf) if nf.ndim == 0 else 0, _ptr(gamma), _ptr(flag), _stream_ptr()))
+    return gamma, flag.bool()
+
+
+def rbf_fold_kernels(G, D, gamma, fold, out=None):
+    """rbf kernels of fold ``fold`` (fcma_rbf_fold_kernels): ``K_fit = exp(-g ((G_aa + G_bb) - 2 G_ab))`` and
+    ``K_pred = exp(-g D)`` with ``g = gamma[item, fold]`` (float64 CUDA ``[n, num_folds]``), written out of place into
+    ``out = (K_fit, K_pred)`` (float64 ``[n, E, E]``, allocated if None) and returned.  The operations of
+    ``feature_kernels_f64_wide``'s rbf epilogue: the same bits for the same gamma."""
+    lib = _lib.load()
+    _check_gd(G, D)
+    n, E, _ = G.shape
+    if gamma.dtype != torch.float64 or gamma.dim() != 2 or gamma.shape[0] != n or not gamma.is_contiguous():
+        raise ValueError("gamma must be contiguous float64 [n, num_folds]")
+    if out is None:
+        out = (torch.empty_like(G), torch.empty_like(G))
+    K_fit, K_pred = out
+    _check_gd(K_fit, K_pred)
+    if K_fit.shape != G.shape:
+        raise ValueError("out must be two float64 [n, E, E] tensors")
+    with torch.cuda.device(G.device):
+        _lib.check(lib.fcma_rbf_fold_kernels(_ptr(G), _ptr(D), n, E, _ptr(gamma), gamma.shape[1], int(fold), _ptr(K_fit),
+                                             _ptr(K_pred), _stream_ptr()))
+    return K_fit, K_pred
+
+
+def svm_cv_scale(G, D, moments, nfeat, labels, num_folds, C=1.0, tol=1e-3, max_iter=-1, shrinking=True, folds=None,
+                 return_iters=False):
+    """Mean cross-validation accuracy of ``SVC(kernel='rbf', gamma='scale', C, tol, shrinking)`` for every item of a
+    block of ``feature_gram_wide`` / ``searchlight_gram_wide`` outputs (``nfeat`` features, a number or one per item):
+    per fold f, the gamma of the fold's training samples (``fold_gammas``), that fold's kernels (``rbf_fold_kernels``, one
+    ``[n, E, E]`` pair reused from fold to fold) and the fp64 solver on that fold's problems only; the ``[n, num_folds]``
+    accuracies are averaged as ``cross_val_score(...).mean()``.  ``folds``: ``svm_folds_for`` problems (the default).
+    Returns ``(acc, flagged)``: float64 ``[n]`` and the bool ``[n]`` mask of items whose gamma may differ from
+    scikit-learn's (``fold_gammas``) -- score those on the host.  ``return_iters``: also the int32 ``[n, nproblems]``
+    iteration counts."""
+    lib = _lib.load()
+    _check_gd(G, D)
+    n, E, _ = G.shape
+    if folds is None:
+        folds = svm_folds_for(labels, num_folds, E)
+    gamma, flag = fold_gammas(moments, fold_train_mask(folds, E), nfeat)
+    solve = lib.fcma_svm_cv_solve_f64_wide if folds.wide else lib.fcma_svm_cv_solve_f64
+    out = (torch.empty_like(G), torch.empty_like(G))
+    correct, iters = [], []
+    for f in range(folds.num_folds):
+        K_fit, K_pred = rbf_fold_kernels(G, D, gamma, f, out=out)
+        c, it = _svm_correct(solve, (_ptr(K_fit), _ptr(K_pred)), K_fit, C, tol, max_iter, shrinking,
+                             fold_problems(folds, f), return_iters)
+        correct.append(c)
+        iters.append(it)
+    scores = torch.cat(correct, dim=1).cpu().numpy().astype(np.float64) / folds.n_test[None, :]
+    acc = scores.mean(axis=1)
+    flagged = flag.any(dim=1).cpu().numpy()
+    if return_iters:
+        return acc, flagged, torch.cat(iters, dim=1).cpu().numpy()
+    return acc, flagged
 
 
 # ------------------------------------------------------------------ searchlight (MVPAVoxelSelector)
@@ -931,3 +1088,30 @@ def _searchlight_kernels(entry, vol, mask, sl_rad, shape, centres, kind, gamma):
                          M, kcode, g.ctypes.data_as(ctypes.c_void_p) if g is not None else None, _ptr(K_fit),
                          _ptr(K_pred) if kcode == 1 else None, _stream_ptr()))
     return K_fit, K_pred
+
+
+def searchlight_gram_wide(vol, mask, sl_rad, shape, centres):
+    """The fp64 sums behind ``SVC(kernel='rbf', gamma='scale')`` on searchlight centres (fcma_searchlight_gram_wide, the
+    arguments of ``searchlight_kernels_wide``, 1 <= E <= 256): ``(G, D, moments)``, G and D float64 ``[M, E, E]`` -- the
+    entries ``searchlight_kernels_wide(kind='rbf')`` exponentiates, bit for bit -- and ``moments`` float64 ``[M, E, 4]``,
+    the double-double sums (s.hi, s.lo, q.hi, q.lo) of each epoch's features and their squares in cube order."""
+    if vol.dim() != 4 or vol.dtype != torch.float32 or not vol.is_contiguous():
+        raise ValueError("vol must be a contiguous float32 [X, Y, Z, E] tensor")
+    X, Y, Z, E = vol.shape
+    if tuple(mask.shape) != (X, Y, Z):
+        raise ValueError("mask shape %s does not match the volume %s" % (tuple(mask.shape), (X, Y, Z)))
+    side = 2 * int(sl_rad) + 1
+    if tuple(shape.shape) != (side, side, side):
+        raise ValueError("shape must be (2*sl_rad+1)^3")
+    mask = mask.to(device=vol.device, dtype=torch.uint8).contiguous()
+    shape = shape.to(device=vol.device, dtype=torch.uint8).contiguous()
+    c = np.ascontiguousarray(centres, dtype=np.int64)
+    M = len(c)
+    G = torch.empty((M, E, E), dtype=torch.float64, device=vol.device)
+    D = torch.empty_like(G)
+    moments = torch.empty((M, E, 4), dtype=torch.float64, device=vol.device)
+    with torch.cuda.device(vol.device):
+        _lib.check(_lib.load().fcma_searchlight_gram_wide(_ptr(vol), X, Y, Z, E, _ptr(mask), int(sl_rad), _ptr(shape),
+                                                          c.ctypes.data_as(ctypes.c_void_p), M, _ptr(G), _ptr(D),
+                                                          _ptr(moments), _stream_ptr()))
+    return G, D, moments

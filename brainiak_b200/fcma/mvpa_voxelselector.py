@@ -9,8 +9,11 @@ For ``SVC(kernel='linear')`` and ``SVC(kernel='rbf')`` with ``gamma='auto'`` or 
 GPU for up to 256 epochs: k_searchlight_kernels (k_searchlight_kernels_tiled above 32 epochs) builds each centre's fp64
 kernel matrices and the batched libsvm SMO restatement cross-validates them in fp64 (engine.svm_cv_f64, on
 ``engine.svm_folds_for`` folds: its wide form above 64 epochs).  libsvm keeps Q in float but QD and the decision values
-in double, so fp64 kernels give the same iterations and predictions as scikit-learn on the features (DESIGN.md).  Any
-other classifier (``gamma='scale'``, poly, sigmoid, other estimators), float64 data, more than 256 epochs, folds the
+in double, so fp64 kernels give the same iterations and predictions as scikit-learn on the features (DESIGN.md).
+scikit-learn's default ``SVC()`` (rbf with ``gamma='scale'``, a gamma per centre and fold) runs there as well:
+engine.searchlight_gram_wide gives each centre's G, D and per-sample moments once, and engine.svm_cv_scale derives every
+fold's gamma and kernels from them; a centre whose exact variance NumPy's may miss by more than a few ulps is scored on
+the host.  Any other classifier (poly, sigmoid, other estimators), float64 data, more than 256 epochs, folds the
 solver cannot express or ``gpu_cv=False`` run the reference's per-centre ``cross_val_score`` on the host.
 """
 import logging
@@ -62,7 +65,7 @@ class MVPAVoxelSelector:
     gpu_cv: score eligible SVC classifiers on the GPU (default; up to 256 epochs); ``False`` -> the reference's host
         loop
     batch_centres: centres per GPU batch (default: sized to free device memory; a centre's kernel matrices take
-        8 E^2 bytes, twice that for rbf)
+        8 E^2 bytes, twice that for rbf, four times for ``gamma='scale'``: G, D and one fold's two kernels)
     """
 
     def __init__(self, data, mask, labels, num_folds, sl, *, device=None, gpu_cv=True, batch_centres=None):
@@ -82,11 +85,14 @@ class MVPAVoxelSelector:
 
     # ------------------------------------------------------------------ routing
     def _gpu_kind(self, clf):
-        """'linear' / 'rbf' if ``clf`` and the data can be scored on the GPU, else None."""
+        """'linear' / 'rbf' / 'scale' (rbf with gamma='scale') if ``clf`` and the data can be scored on the GPU, else
+        None."""
         if not self.gpu_cv:
             return None
-        kind = engine.svc_feature_kind(clf, self.labels, self.num_folds, self.data.shape[3],
-                                       max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
+        E = self.data.shape[3]
+        kind = engine.svc_feature_kind(clf, self.labels, self.num_folds, E, max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
+        if kind is None and engine.svc_scale_supported(clf, self.labels, self.num_folds, E):
+            kind = 'scale'
         if kind is not None and np.asarray(self.data).dtype != np.float32:
             logger.info('MVPAVoxelSelector: data is %s, not float32: scoring on the host', np.asarray(self.data).dtype)
             return None
@@ -143,17 +149,18 @@ class MVPAVoxelSelector:
         return result_volume, results
 
     # ------------------------------------------------------------------ host path (the reference's loop)
-    def _run_host(self, clf, centres, shape):
-        data = np.asarray(self.data)
+    def _features(self, c, shape):
+        """The features ``[E, n_features]`` of centre ``c`` (a linear index into the mask), as the reference hands them to
+        the classifier."""
         r = int(self.sl.sl_rad)
         ny, nz = self.mask.shape[1], self.mask.shape[2]
-        out = []
-        for c in centres.tolist():
-            x, y, z = c // (ny * nz), (c // nz) % ny, c % nz
-            sl = np.s_[x - r:x + r + 1, y - r:y + r + 1, z - r:z + r + 1]
-            m = self.mask[sl] * shape
-            out.append(_host_accuracy(clf, data[sl][m, :].T, self.labels, self.num_folds))
-        return out
+        x, y, z = c // (ny * nz), (c // nz) % ny, c % nz
+        sl = np.s_[x - r:x + r + 1, y - r:y + r + 1, z - r:z + r + 1]
+        m = self.mask[sl] * shape
+        return np.asarray(self.data)[sl][m, :].T
+
+    def _run_host(self, clf, centres, shape):
+        return [_host_accuracy(clf, self._features(c, shape), self.labels, self.num_folds) for c in centres.tolist()]
 
     # ------------------------------------------------------------------ GPU path
     def _torch_device(self):
@@ -185,7 +192,7 @@ class MVPAVoxelSelector:
             vol = torch.from_numpy(data).to(dev)
             mask_d = torch.from_numpy(self.mask.astype(np.uint8)).to(dev)
             shape_d = torch.from_numpy(shape.astype(np.uint8)).to(dev)
-            per_centre = E * E * 8 * (2 if kind == 'rbf' else 1)
+            per_centre = E * E * 8 * {'linear': 1, 'rbf': 2, 'scale': 4}[kind]
             if self.batch_centres:
                 batch = int(self.batch_centres)
             else:
@@ -194,6 +201,18 @@ class MVPAVoxelSelector:
             acc = []
             for b0 in range(0, len(centres), batch):
                 cb = centres[b0:b0 + batch]
+                if kind == 'scale':
+                    G, D, moments = engine.searchlight_gram_wide(vol, mask_d, r, shape_d, cb)
+                    a, flagged = engine.svm_cv_scale(G, D, moments, nfeat[b0:b0 + batch], self.labels, self.num_folds,
+                                                     C=clf.C, tol=clf.tol, max_iter=clf.max_iter,
+                                                     shrinking=clf.shrinking, folds=folds)
+                    del G, D, moments
+                    for k in np.flatnonzero(flagged):
+                        a[k] = _host_accuracy(clf, self._features(int(cb[k]), shape), self.labels, self.num_folds)
+                    if flagged.any():
+                        logger.info('%d centres scored on the host (gamma=\'scale\' variance check)', int(flagged.sum()))
+                    acc.append(a)
+                    continue
                 K_fit, K_pred = kernels(vol, mask_d, r, shape_d, cb, kind, gamma[b0:b0 + batch] if kind == 'rbf' else None)
                 acc.append(engine.svm_cv_f64(K_fit, K_pred, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
                                              max_iter=clf.max_iter, shrinking=clf.shrinking, folds=folds))

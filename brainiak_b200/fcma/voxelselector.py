@@ -8,7 +8,8 @@ accuracy, descending), same private stage methods.  The three native stages of
     corr GEMM (TMA + wgmma)  ->  Fisher-z + within-subject z-score  ->  per-voxel E x E kernel
 
 The cross validation runs on the GPU for ``SVC(kernel='precomputed')`` on the kernel matrices and for
-``SVC(kernel='linear' | 'rbf')`` on the normalised correlation vectors (see ``gpu_cv``); any other classifier is
+``SVC(kernel='linear' | 'rbf')`` on the normalised correlation vectors, ``SVC()``'s ``gamma='scale'`` included (see
+``gpu_cv``); any other classifier is
 cross-validated on the host by scikit-learn, exactly as in the reference (voxelselector.py:41-53).  Distribution: instead of the MPI master/worker farm (voxelselector.py:176-282) every
 rank of ``torch.distributed`` owns a contiguous slice of voxel rows (work per row is uniform); the
 per-voxel scores are gathered on ``master_rank``.  Without ``torch.distributed`` it runs on one GPU.
@@ -100,8 +101,12 @@ class VoxelSelector:
         are built on the GPU (engine.feature_kernels_f64, above 64 epochs engine.feature_kernels_f64_wide, without the
         decimal shrink, as scikit-learn sees the features) and cross-validated by engine.svm_cv_f64 (at most 256 epochs
         and 64 folds, no class weights, probability or tie
-        breaking, and ``mask_self=False``, see engine.svc_feature_kind).  ``False`` or any other classifier ->
-        scikit-learn on the host, exactly as the reference (voxelselector.py:41-53)
+        breaking, and ``mask_self=False``, see engine.svc_feature_kind).  scikit-learn's default ``SVC()`` (rbf with
+        ``gamma='scale'``, whose gamma depends on each fold's training features) runs there too under the same limits
+        (engine.svc_scale_supported): G and D of the features and their per-sample moments are built once
+        (engine.feature_gram_wide), then every fold gets its own gamma and kernels (engine.svm_cv_scale); a voxel whose
+        exact variance NumPy's may miss by more than a few ulps is scored on the host.  ``False`` or any other
+        classifier -> scikit-learn on the host, exactly as the reference (voxelselector.py:41-53)
     """
 
     def __init__(self, labels, epochs_per_subj, num_folds, raw_data, raw_data2=None,
@@ -344,9 +349,9 @@ class VoxelSelector:
             results += self._cv_block(K[s - k0:s - k0 + nb], s, nb, clf, on_gpu, folds)
         return results
 
-    def _plain_block(self, n, fp64_outputs=False):
+    def _plain_block(self, n, fp64_outputs=False, fp64_matrices=2):
         """Rows per pass of the plain (row-block) pipeline, with its scratch allocated for them.  ``fp64_outputs``: the
-        pass also holds the rows' fp64 K_fit and K_pred (engine.feature_block_rows)."""
+        pass also holds ``fp64_matrices`` fp64 [E, E] matrices per row (engine.feature_block_rows)."""
         import torch
         rows_op, _ = self._operands()
         E = rows_op.E
@@ -355,7 +360,7 @@ class VoxelSelector:
         else:
             free, _ = torch.cuda.mem_get_info(rows_op.device)
             block = engine.feature_block_rows(E, _lib.load().fcma_work_bytes_per_row(E, self.num_voxels2), n,
-                                              min(free // 2, 32 << 30))
+                                              min(free // 2, 32 << 30), matrices=fp64_matrices)
         block = max(1, min(block, n))
         if self._work is None or self._work.rows < block or isinstance(self._work, engine.SymWorkspace):
             self._work = None
@@ -369,6 +374,38 @@ class VoxelSelector:
         if not self.gpu_cv or self.mask_self:
             return None
         return engine.svc_feature_kind(clf, self.labels, self.num_folds, len(self.raw_data), max_epochs=max_epochs)
+
+    def _scale_ok(self, clf):
+        """True when ``SVC(kernel='rbf', gamma='scale')`` on the normalised correlation vectors is cross-validated on the
+        GPU with per-fold gammas (engine.svm_cv_scale), under the conditions of ``_feature_kind``."""
+        if not self.gpu_cv or self.mask_self:
+            return False
+        return engine.svc_scale_supported(clf, self.labels, self.num_folds, len(self.raw_data))
+
+    def _score_rows_scale(self, start, n, clf):
+        """SVC(kernel='rbf', gamma='scale') on the features of rows [start, start+n): G, D and the per-sample moments of
+        every row (engine.feature_gram_wide), then per fold the gamma of its training samples, its rbf kernels and the fp64
+        solver (engine.svm_cv_scale).  The voxels whose gamma may differ from scikit-learn's are scored on the host."""
+        rows_op, cols_op = self._operands()
+        E = rows_op.E
+        folds = engine.svm_folds_for(self.labels, self.num_folds, E)
+        block = self._plain_block(n, fp64_outputs=True, fp64_matrices=4)
+        results = []
+        for s in range(start, start + n, block):
+            nb = min(block, start + n - s)
+            G, D, moments = engine.feature_gram_wide(rows_op, cols_op, s, nb, self.epochs_per_subj, work=self._work)
+            acc, flagged = engine.svm_cv_scale(G, D, moments, self.num_voxels2, self.labels, self.num_folds, C=clf.C,
+                                               tol=clf.tol, max_iter=clf.max_iter, shrinking=bool(clf.shrinking),
+                                               folds=folds)
+            del G, D, moments
+            part = [(int(s + k), acc[k]) for k in range(nb)]
+            for k in np.flatnonzero(flagged):
+                part[k] = self._voxel_scoring((int(s + k), 1), clf)[0]
+            if flagged.any():
+                logger.info('rows [%d, %d): %d voxels scored on the host (gamma=\'scale\' variance check)', s, s + nb,
+                            int(flagged.sum()))
+            results += part
+        return results
 
     def _score_rows(self, start, n, clf):
         """GPU stages for rows [start, start+n) in HBM-sized blocks, then the cross validation (GPU or host)."""
@@ -406,6 +443,8 @@ class VoxelSelector:
                 K = engine.voxel_kernels(rows_op, cols_op, s, nb, self.epochs_per_subj,
                                          flags=self._flags(fused), work=self._work)
                 results += self._cv_block(K, s, nb, clf, on_gpu, folds)
+        elif self._scale_ok(clf):
+            results = self._score_rows_scale(start, n, clf)
         else:
             unit = max(1, min(self.voxel_unit, n))
             for s in range(start, start + n, unit):

@@ -278,6 +278,30 @@ int fcma_voxel_feature_kernels_wide(const void *rows_op, const void *cols_op, in
                                     long start, long nb, int eps, int kind, double gamma, float *work_dev,
                                     size_t work_bytes, double *K_fit_dev, double *K_pred_dev, void *stream);
 
+/* ---- SVC(kernel='rbf', gamma='scale'): gamma = 1 / (F var(X_train)) per (item, fold) ---------------------------------
+ * fcma_voxel_feature_kernels_wide's pipeline without the rbf epilogue: G_dev = G, D_dev = D (double [nb][E][E], the
+ * entries fcma_voxel_feature_kernels_wide exponentiates), and moments_dev = double [nb][E][4]: s.hi, s.lo, q.hi, q.lo of
+ * the double-double sums s_e = sum_j z_ej, q_e = sum_j z_ej^2 over the row's normalised features (fixed order).
+ * 1 <= E <= 256. */
+int fcma_voxel_feature_gram_wide(const void *rows_op, const void *cols_op, int precision, int E, int T, long V, long V2,
+                                 long start, long nb, int eps, float *work_dev, size_t work_bytes, double *G_dev,
+                                 double *D_dev, double *moments_dev, void *stream);
+/* the same for searchlight centres (arguments of fcma_searchlight_kernels_wide): G and D as fcma_searchlight_kernels_wide
+ * sums them, not exponentiated, and the moments of each centre's features in cube order.  1 <= E <= 256. */
+int fcma_searchlight_gram_wide(const float *vol_dev, long nx, long ny, long nz, int E, const unsigned char *mask_dev,
+                               int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, double *G_dev,
+                               double *D_dev, double *moments_dev, void *stream);
+/* gamma_dev[item][fold] = scikit-learn's gamma='scale' on the fold's training samples (train_host: bytes [nfolds][E], 1 =
+ * training sample): 1 / (F * var) with var the exact variance of the n_train x F training features rounded once, 1.0 if
+ * var == 0.  F = nfeat_dev[item] (int64, device) or, if nfeat_dev is null, nfeat.  flag_dev[item][fold] = 1 where
+ * NumPy's two-pass variance may differ from var by more than a few ulps (mean^2 > 2^36 var; DESIGN.md §3.9). */
+int fcma_fold_gammas(const double *moments_dev, long n, int E, int nfolds, const unsigned char *train_host,
+                     const long *nfeat_dev, long nfeat, double *gamma_dev, unsigned char *flag_dev, void *stream);
+/* rbf kernels of one fold, out of place: K_fit = exp(-g ((G_aa + G_bb) - 2 G_ab)), K_pred = exp(-g D) with
+ * g = gamma_dev[item * nfolds + fold]; the operations of fcma_voxel_feature_kernels_wide's rbf epilogue. */
+int fcma_rbf_fold_kernels(const double *G_dev, const double *D_dev, long n, int E, const double *gamma_dev, int nfolds,
+                          int fold, double *K_fit_dev, double *K_pred_dev, void *stream);
+
 /* ---- a12 / a15: plain NT GEMM  C[m][n] = sum_k A[m][k]*B[n][k]  (fp32 FFMA, row-major) ---------- */
 int fcma_gemm_nt(const float *A_dev, const float *B_dev, float *C_dev, long M, long N, long K,
                  long lda, long ldb, long ldc, void *stream);
