@@ -21,6 +21,9 @@
  *     (e.g. torch.Tensor.data_ptr()); `stream` is a cudaStream_t passed as void* (0 = default).
  *   - The caller owns every buffer (as in the reference, voxelselector.py:307, classifier.py:166);
  *     the library never retains pointers across calls.
+ *   - An entry point writes only the outputs it documents, within their documented extents, and never writes its
+ *     const inputs or host arrays; every copy, memset, scratch allocation and launch it issues (uploads of host arrays
+ *     such as fold structs, centres, gammas and training masks included) goes on `stream`.
  *   - Return value: 0 on success, negative FCMA_E* on failure; fcma_last_error() returns a
  *     thread-local message.  (Reference: ValueError from Cython memoryviews, RuntimeError from
  *     fcma_extension.cc:47 — the Python wrapper maps FCMA_EINVAL->ValueError, others->RuntimeError.)
@@ -158,10 +161,10 @@ int fcma_voxel_kernels(const void *rows_op, const void *cols_op, int precision, 
  * rows [start, start+nb) are contracted with columns [start, V) only and every block is used twice, for its row
  * voxels and (transposed) for its column voxels.  K_dev is the FULL [V][E][E] array and is ACCUMULATED into
  * (caller zeroes it): after this call K[i] (start <= i < start+nb) holds the columns j >= start, and K[j]
- * (j >= start+nb) has received the columns in [start, start+nb).  Calling it once with (0, V), or once per shard
- * of a partition of [0, V) -- e.g. one shard per GPU followed by a sum (all-reduce) of the K arrays -- yields the
- * same kernels as fcma_voxel_kernels.  nb must be a multiple of 256 unless start+nb == V; eps a power of two
- * (fused path); work_dev must hold at least 256 rows (see fcma_sym_rows_per_pass). */
+ * (j >= start+nb) has received the columns in [start, start+nb); rows i < start are not touched.  Calling it once
+ * with (0, V), or once per shard of a partition of [0, V) -- e.g. one shard per GPU followed by a sum (all-reduce) of
+ * the K arrays -- yields the same kernels as fcma_voxel_kernels.  nb must be a multiple of 256 unless start+nb == V;
+ * eps a power of two (fused path); work_dev must hold at least 256 rows (see fcma_sym_rows_per_pass). */
 int fcma_voxel_kernels_sym(const void *op, int precision, int E, int T, long V, long start, long nb, int eps,
                            int flags, float *work_dev, size_t work_bytes, float *K_dev, void *stream);
 /* The same for epochs that are still arriving (multi-GPU input exchange): epochs_dev receives `ngroups` contiguous epoch
@@ -213,7 +216,8 @@ int fcma_svm_cv_precomputed(const float *K_dev, long nv, int E, int nfolds, cons
 
 /* the general form of the solver.  shrinking != 0: libsvm's shrinking heuristic restated as well (do_shrinking, be_shrunk,
  * reconstruct_gradient, the counter / unshrink logic of Solver::Solve) = scikit-learn's default SVC(shrinking=True).
- * correct_dev and bits_dev are both optional (at least one): bit t of bits_dev[v*nproblems + p] is set when sample test_idx[t]
+ * correct_dev and bits_dev are both optional (at least one), iters_dev as well; a null output is not written and the
+ * others do not depend on which are given: bit t of bits_dev[v*nproblems + p] is set when sample test_idx[t]
  * of problem p falls on the side of the first (smaller-label) class.  One struct per (fold, class pair) gives one-vs-one
  * multi-class cross-validation (votes as in libsvm's svm_predict: first maximum wins). */
 int fcma_svm_cv_solve(const float *K_dev, long nv, int E, int nproblems, const void *folds_host, double C, double tol,
@@ -245,8 +249,9 @@ int fcma_svm_cv_solve_f64_wide(const double *K_fit_dev, const double *K_pred_dev
  * vol_dev: float32 [nx][ny][nz][E] (epochs contiguous per voxel); mask_dev: bytes [nx][ny][nz]; shape_dev: bytes
  * [2r+1]^3; centres_host: M linear voxel indices, each at least sl_rad from every face; the features of a centre are
  * the voxels of its cube where mask and shape hold, in C order.  K_fit_dev (and K_pred_dev for rbf): double [M][E][E].
- * kind 0 linear: K_fit = G = sum_f x_a x_b.  kind 1 rbf with gamma_host[M]: K_fit = exp(-gamma ((G_aa + G_bb) - 2 G_ab)),
- * K_pred = exp(-gamma sum_f (x_a - x_b)^2).  fp64 sums in cube order, no FMA contraction.  1 <= E <= 64. */
+ * kind 0 linear: K_fit = G = sum_f x_a x_b (K_pred_dev may be null; a separate K_pred is not written).  kind 1 rbf
+ * with gamma_host[M]: K_fit = exp(-gamma ((G_aa + G_bb) - 2 G_ab)), K_pred = exp(-gamma sum_f (x_a - x_b)^2).  fp64
+ * sums in cube order, no FMA contraction.  1 <= E <= 64. */
 int fcma_searchlight_kernels(const float *vol_dev, long nx, long ny, long nz, int E, const unsigned char *mask_dev,
                              int sl_rad, const unsigned char *shape_dev, const long *centres_host, long M, int kind,
                              const double *gamma_host, double *K_fit_dev, double *K_pred_dev, void *stream);
@@ -262,7 +267,7 @@ int fcma_searchlight_kernels_wide(const float *vol_dev, long nx, long ny, long n
  * second stage.  For voxel rows [start, start+nb): z[i] = the raw correlations r[i] ([E][V2]) normalised exactly as
  * fcma_within_subject_norm does (any eps >= 1; epochs past the last whole subject keep their raw r), then, in fp64,
  * G_ab = sum_j z_aj z_bj and, for rbf, D_ab = sum_j (z_aj - z_bj)^2, in a fixed order (two runs are bit-identical).
- *   kind 0 linear: K_fit = G (K_pred_dev may be null).
+ *   kind 0 linear: K_fit = G (K_pred_dev may be null; a separate K_pred is not written).
  *   kind 1 rbf:    K_fit = exp(-gamma ((G_aa + G_bb) - 2 G_ab)), K_fit_aa = 1; K_pred = exp(-gamma D).  gamma >= 0, finite.
  * These are the kernel values libsvm computes for SVC(kernel=...) on the float32 features z[i], so fcma_svm_cv_solve_f64
  * on them cross-validates that classifier.  Outputs double [nb][E][E]; 1 <= E <= 64. */
