@@ -67,6 +67,8 @@ SIGNATURES = {
     "fcma_classifier_kernel_sym": (c_int, [c_void_p, c_int, c_int, c_int, c_long, c_int, c_int, c_void_p, c_size_t, c_void_p,
                                            c_void_p]),
     "fcma_shrink_kernels": (c_int, [c_void_p, c_long, c_int, c_void_p, c_void_p]),
+    "fcma_subset_kernels": (c_int, [c_void_p, c_long, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "fcma_subset_kernels_f64": (c_int, [c_void_p, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fcma_svm_cv_precomputed": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double,
                                         ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p]),
     "fcma_svm_cv_solve": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, ctypes.c_double, ctypes.c_double, c_int, c_int,

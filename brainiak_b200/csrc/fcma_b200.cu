@@ -21,6 +21,7 @@
 #include <string.h>
 #include <type_traits>
 
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 
@@ -3438,7 +3439,7 @@ extern "C" int fcma_row_normalize(float *X_dev, long R, long D, long ld, int nan
 // trunc(|f|) >= N <=> |f| >= N, and for N = 10^k that holds exactly when |f| >= the smallest float32 >= 10^k (the table,
 // generated with Python integers and checked by tests/test_gpu_pack_and_side_kernels.py).  A negative value with
 // int() != 0 adds one for the '-' sign.  NaN and +-inf, where the reference's int() raises, give nd = 1: K untouched.
-__global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E, int *digits_out)
+__device__ __forceinline__ int shrink_digits(float k00)
 {
     constexpr float kPow10Ceil[38] = {
         0x1.400000p+3f, 0x1.900000p+6f, 0x1.f40000p+9f, 0x1.388000p+13f, 0x1.86a000p+16f, 0x1.e84800p+19f,
@@ -3449,11 +3450,6 @@ __global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E
         0x1.f8defap+102f, 0x1.3b8b5cp+106f, 0x1.8a6e34p+109f, 0x1.ed09c0p+112f, 0x1.342618p+116f, 0x1.812f9ep+119f,
         0x1.e17b86p+122f, 0x1.2ced34p+126f,
     };  // kPow10Ceil[k - 1] = smallest float32 >= 10^k
-    const long v = (long)blockIdx.x * 4 + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (v >= nv) return;
-    float *Kv = K + (size_t)v * E * E;
-    const float k00 = Kv[0];
     int nd = 1;
     if (isfinite(k00)) {
         const float a = fabsf(k00);
@@ -3461,11 +3457,107 @@ __global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E
         for (int k = 0; k < 38; k++) nd += a >= kPow10Ceil[k];
         if (k00 <= -1.0f) nd++;         // the '-' sign counts in len(str(.)); int(-0.5) is 0
     }
+    return nd;
+}
+
+// float32(10**(2-nd)), the factor of a kernel with nd > 2 digits
+__device__ __forceinline__ float shrink_factor(int nd) { return (float)pow(10.0, (double)(2 - nd)); }
+
+__global__ void __launch_bounds__(128) k_shrink_kernels(float *K, long nv, int E, int *digits_out)
+{
+    const long v = (long)blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (v >= nv) return;
+    float *Kv = K + (size_t)v * E * E;
+    const int nd = shrink_digits(Kv[0]);
     if (digits_out && lane == 0) digits_out[v] = nd;
     if (nd > 2) {
-        const float prop = (float)pow(10.0, (double)(2 - nd));   // float32(10**(2-nd))
+        const float prop = shrink_factor(nd);
         for (int idx = lane; idx < E * E; idx += 32) Kv[idx] *= prop;
     }
+}
+
+// The kernels of a subset of the epochs: out[v][a][b] = K[v][keep[a]][keep[b]], [nv][Ek][Ek] contiguous, optionally with
+// the decimal shrink of k_shrink_kernels counted on the compacted K00 = K[v][keep[0]][keep[0]].  A pure HBM stream: the
+// keep list travels by value (KeepList) and is staged in shared memory; each CTA owns VPC consecutive voxels and its
+// warps walk their Ek output rows, a row split over W = min(32, pow2ceil(Ek)) lanes (32 / W rows per warp at a time),
+// reading the kept elements of the source row (a contiguous run of E) and writing the output row contiguously.
+struct KeepList {
+    int idx[256];
+};
+
+template <typename T, bool SHRINK>
+__global__ void __launch_bounds__(256) k_subset_kernels(const T *__restrict__ K, long nv, int E,
+                                                        const __grid_constant__ KeepList keep, int Ek, int vpc,
+                                                        int lw_log2, T *__restrict__ out, int *digits_out)
+{
+    __shared__ int s_keep[256];
+    __shared__ float s_prop[32];
+    for (int i = threadIdx.x; i < Ek; i += blockDim.x) s_keep[i] = keep.idx[i];
+    const long v0 = (long)blockIdx.x * vpc;
+    const int nvb = (int)min((long)vpc, nv - v0);
+    if constexpr (SHRINK) {
+        if (threadIdx.x < nvb) {
+            const long k0 = (long)keep.idx[0];
+            const int nd = shrink_digits(K[(size_t)(v0 + threadIdx.x) * E * E + k0 * E + k0]);
+            if (digits_out) digits_out[v0 + threadIdx.x] = nd;
+            s_prop[threadIdx.x] = nd > 2 ? shrink_factor(nd) : 0.0f;      // 0: leave the kernel untouched
+        }
+    }
+    __syncthreads();
+    const int lw = 1 << lw_log2, sub = (threadIdx.x & 31) >> lw_log2, l = threadIdx.x & (lw - 1);
+    const int rows_per_pass = (blockDim.x >> 5) << (5 - lw_log2);
+    const int rows = nvb * Ek;
+    for (int r = (threadIdx.x >> 5) * (32 >> lw_log2) + sub; r < rows; r += rows_per_pass) {
+        const int vl = r / Ek, a = r - vl * Ek;
+        const T *src = K + (size_t)(v0 + vl) * E * E + (size_t)s_keep[a] * E;
+        T *dst = out + ((size_t)(v0 + vl) * Ek + a) * Ek;
+        float prop = 0.0f;
+        if constexpr (SHRINK) prop = s_prop[vl];
+        for (int b = l; b < Ek; b += lw) {
+            T x = src[s_keep[b]];
+            if constexpr (SHRINK) {
+                if (prop != 0.0f) x *= prop;
+            }
+            dst[b] = x;
+        }
+    }
+}
+
+template <typename T>
+static int subset_kernels_impl(const char *who, const T *K_dev, long nv, int E, const int *keep_host, int E_keep,
+                               T *out_dev, int shrink, int *digits_dev, void *stream)
+{
+    int rc = check_device();
+    if (rc) return rc;
+    if (!K_dev || !out_dev || !keep_host) return fail(FCMA_EINVAL, "%s: null pointer", who);
+    if (nv <= 0 || E < 1 || E > 256 || E_keep < 1 || E_keep > E)
+        return fail(FCMA_EINVAL, "%s: bad shape nv=%ld E=%d E_keep=%d (1 <= E_keep <= E <= 256)", who, nv, E, E_keep);
+    KeepList keep;
+    for (int a = 0; a < E_keep; a++) {
+        if (keep_host[a] < 0 || keep_host[a] >= E || (a > 0 && keep_host[a] <= keep_host[a - 1]))
+            return fail(FCMA_EINVAL, "%s: keep[%d] = %d: the indices must increase strictly within [0, %d)", who, a,
+                        keep_host[a], E);
+        keep.idx[a] = keep_host[a];
+    }
+    for (int a = E_keep; a < 256; a++) keep.idx[a] = 0;
+    const uintptr_t in0 = (uintptr_t)K_dev, in1 = in0 + (size_t)nv * E * E * sizeof(T);
+    const uintptr_t o0 = (uintptr_t)out_dev, o1 = o0 + (size_t)nv * E_keep * E_keep * sizeof(T);
+    if (o0 < in1 && in0 < o1) return fail(FCMA_EINVAL, "%s: the output overlaps the input", who);
+    // at least 32 output rows per CTA; a row over the fewest power-of-two lanes that cover it
+    const int vpc = (int)std::min<long>(nv, cdiv(32, E_keep));
+    int lw_log2 = 0;
+    while ((1 << lw_log2) < std::min(E_keep, 32)) lw_log2++;
+    const long grid = cdiv(nv, vpc);
+    if (grid > 0x7fffffffL) return fail(FCMA_EINVAL, "%s: too many kernels in one call", who);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if constexpr (std::is_same<T, float>::value) {
+        if (shrink)
+            return launch_kernel(k_subset_kernels<T, true>, (unsigned)grid, 256, 0, st, "k_subset_kernels", K_dev, nv,
+                                 E, keep, E_keep, vpc, lw_log2, out_dev, digits_dev);
+    }
+    return launch_kernel(k_subset_kernels<T, false>, (unsigned)grid, 256, 0, st, "k_subset_kernels", K_dev, nv, E, keep,
+                         E_keep, vpc, lw_log2, out_dev, (int *)nullptr);
 }
 
 // Batched C-SVC cross-validation on precomputed kernels: one warp per (voxel, fold).
@@ -4074,6 +4166,19 @@ extern "C" int fcma_shrink_kernels(float *K_dev, long nv, int E, int *digits_dev
     k_shrink_kernels<<<(unsigned)cdiv(nv, 4), 128, 0, (cudaStream_t)stream>>>(K_dev, nv, E, digits_dev);
     LAUNCH_CHECK("k_shrink_kernels");
     return FCMA_OK;
+}
+
+extern "C" int fcma_subset_kernels(const float *K_dev, long nv, int E, const int *keep_host, int E_keep, float *out_dev,
+                                   int shrink, int *digits_dev, void *stream)
+{
+    return subset_kernels_impl("fcma_subset_kernels", K_dev, nv, E, keep_host, E_keep, out_dev, shrink, digits_dev,
+                               stream);
+}
+
+extern "C" int fcma_subset_kernels_f64(const double *K_dev, long nv, int E, const int *keep_host, int E_keep,
+                                       double *out_dev, void *stream)
+{
+    return subset_kernels_impl("fcma_subset_kernels_f64", K_dev, nv, E, keep_host, E_keep, out_dev, 0, nullptr, stream);
 }
 
 template <typename KT, typename Fold>

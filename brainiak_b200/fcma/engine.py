@@ -643,6 +643,38 @@ def shrink_kernels_(K, return_digits=False):
     return digits
 
 
+def subset_kernels(K, keep, shrink=False, out=None, return_digits=False):
+    """The kernels of the epochs ``keep`` (strictly increasing indices into [0, E), E <= 256):
+    ``out[v] = K[v][keep][:, keep]`` for contiguous CUDA ``K`` ``[nv, E, E]``, float32 (fcma_subset_kernels) or float64
+    (fcma_subset_kernels_f64), written out of place into ``out`` (``[nv, len(keep), len(keep)]`` of K's dtype,
+    allocated if None) and returned.  ``shrink`` (float32 only): ``shrink_kernels_`` in the same pass, its digits counted
+    on the compacted ``out[v, 0, 0]``; ``return_digits``: also those digit counts, int32 ``[nv]``."""
+    lib = _lib.load()
+    if K.dim() != 3 or K.shape[1] != K.shape[2] or not K.is_contiguous() or K.dtype not in (torch.float32, torch.float64):
+        raise ValueError("K must be contiguous float32 or float64 [nv, E, E]")
+    f64 = K.dtype == torch.float64
+    if f64 and (shrink or return_digits):
+        raise ValueError("the decimal shrink applies to float32 kernels only")
+    keep_h = np.ascontiguousarray(keep, dtype=np.int32)
+    if keep_h.ndim != 1:
+        raise ValueError("keep must be a 1-D list of epoch indices")
+    nv, E, _ = K.shape
+    Ek = len(keep_h)
+    if out is None:
+        out = torch.empty((nv, Ek, Ek), dtype=K.dtype, device=K.device)
+    elif out.shape != (nv, Ek, Ek) or out.dtype != K.dtype or out.device != K.device or not out.is_contiguous():
+        raise ValueError("out must be contiguous [%d, %d, %d] of K's dtype and device" % (nv, Ek, Ek))
+    digits = torch.empty(nv, dtype=torch.int32, device=K.device) if return_digits else None
+    kp = keep_h.ctypes.data_as(ctypes.c_void_p)
+    with torch.cuda.device(K.device):
+        if f64:
+            _lib.check(lib.fcma_subset_kernels_f64(_ptr(K), nv, E, kp, Ek, _ptr(out), _stream_ptr()))
+        else:
+            _lib.check(lib.fcma_subset_kernels(_ptr(K), nv, E, kp, Ek, _ptr(out), 1 if shrink else 0,
+                                               _ptr(digits) if digits is not None else None, _stream_ptr()))
+    return (out, digits) if return_digits else out
+
+
 def svm_cv_supported(clf, labels, num_folds, E, allow_shrinking=True, max_epochs=64):
     """True if ``cross_val_score(clf, K, labels, cv=StratifiedKFold(num_folds))`` can run on the GPU:
     ``SVC(kernel='precomputed')`` without class weights / probability / tie breaking, E <= ``max_epochs`` (64, or up to

@@ -57,6 +57,30 @@ def _is_precomputed_svc(clf):
     return isinstance(clf, sklearn.svm.SVC) and clf.kernel == 'precomputed'
 
 
+def held_out_keep(E, epochs_per_subj, subject):
+    """The epochs left when ``subject`` is held out: ``[0, E)`` without ``[subject * eps, (subject + 1) * eps)``, in the
+    original order (the reference example's ``subsampled_idx``, fcma_voxel_selection_cv.py:69-75)."""
+    s0 = subject * epochs_per_subj
+    return np.concatenate([np.arange(0, s0), np.arange(s0 + epochs_per_subj, E)]).astype(np.int64)
+
+
+class _Case:
+    """One cross validation of a kernel build: ``run()``'s over every epoch (``keep`` None), or that of a run without one
+    held-out subject (``keep``: the epochs left), with that run's labels and fold count."""
+
+    def __init__(self, E, labels, num_folds, keep=None):
+        self.keep, self.labels, self.num_folds = keep, labels, num_folds
+        self.E = E if keep is None else len(keep)
+
+    def take(self, x, axes):
+        """The host array ``x`` restricted to the kept epochs along ``axes`` (``x`` itself for every epoch)."""
+        if self.keep is None:
+            return x
+        for ax in axes:
+            x = np.take(x, self.keep, axis=ax)
+        return x
+
+
 def shrink_kernels_(kernels):
     """In-place decimal shrink of every ``[E, E]`` kernel (reference voxelselector.py:409-412):
     ``nd = len(str(int(K[i, 0, 0]))); if nd > 2: K[i] *= 10**(2 - nd)``."""
@@ -240,6 +264,84 @@ class VoxelSelector:
             return results
         return []
 
+    def held_out_cases(self, subjects=None, num_folds=None):
+        """The leave-one-subject-out runs of ``run_held_out``: one ``_Case`` per subject of ``subjects`` (default: every
+        subject), with ``labels_s`` and ``num_folds`` (default: subjects - 1).  Raises ValueError before any device is
+        touched when E is not a whole number of subjects, there are fewer than 3 subjects, or ``subjects`` holds an index
+        outside [0, S) or a duplicate."""
+        E, eps = len(self.raw_data), int(self.epochs_per_subj)
+        if eps < 1 or E % eps:
+            raise ValueError('leave-one-subject-out needs whole subjects: %d epochs are not a multiple of '
+                             'epochs_per_subj = %d' % (E, eps))
+        S = E // eps
+        if S < 3:
+            raise ValueError('leave-one-subject-out needs at least 3 subjects, not %d' % S)
+        subjects = list(range(S)) if subjects is None else [int(x) for x in subjects]
+        if any(x < 0 or x >= S for x in subjects) or len(set(subjects)) != len(subjects):
+            raise ValueError('subjects must be distinct indices in [0, %d): %r' % (S, subjects))
+        num_folds = S - 1 if num_folds is None else int(num_folds)
+        cases = []
+        for x in subjects:
+            keep = held_out_keep(E, eps, x)
+            cases.append(_Case(E, [self.labels[i] for i in keep], num_folds, keep))
+        return subjects, cases
+
+    def run_held_out(self, clf, subjects=None, num_folds=None):
+        """Leave-one-subject-out voxel selection from one kernel build.
+
+        The reference's FCMA example (fcma_voxel_selection_cv.py) runs the whole selection once per held-out subject s:
+        ``VoxelSelector(labels_s, eps, num_folds, raw_s, raw2_s, ...).run(clf)``, ``_s`` meaning the epochs
+        ``[s * eps, (s + 1) * eps)`` removed.  The correlations, their within-subject z-scores and every kernel entry of
+        the other subjects do not depend on subject s, so here every row block's kernels are built once over all E epochs,
+        by the code ``run()`` uses, and each held-out run compacts them to its E - eps epochs on the device
+        (engine.subset_kernels, with the decimal shrink counted on the compacted K00) before the cross validation
+        ``run()`` would do with ``labels_s`` and ``svm_folds_for(labels_s, num_folds, E - eps)``.  The host routes
+        take the same block with subject s's epochs sliced out.
+
+        ``subjects``: the held-out subjects (default: all ``S = E // epochs_per_subj``); ``num_folds``: the inner fold
+        count (default ``S - 1``, the example's ``num_subjs - 1``).  Returns ``{s: [(voxel_id, accuracy), ...]}``, each
+        list sorted as ``run()`` sorts, on ``master_rank`` and ``{}`` elsewhere; equal to the per-subject ``run()``
+        lists.  The precision is resolved once over all E epochs (``_operands``): when a subset alone would resolve to
+        another split mode, the kernels agree within the fp32-faithful tolerance instead of bit for bit."""
+        subjects, cases = self.held_out_cases(subjects, num_folds)
+        rank, world = self._world()
+        start, n = self.row_partition(self.num_voxels, world)[rank]
+        time1 = time.time()
+        local = self._score_cases(start, n, clf, cases) if n > 0 else [[] for _ in cases]
+        logger.info('rank %d scored rows [%d, %d) for %d held-out subjects in %.2f s', rank, start, start + n,
+                    len(cases), time.time() - time1)
+        results = self._gather_held_out(local, rank, world)
+        if rank != self.master_rank:
+            return {}
+        out = {}
+        for x, res in zip(subjects, results):
+            res.sort(key=lambda tup: tup[1], reverse=True)
+            out[x] = res
+        return out
+
+    def _gather_held_out(self, local, rank, world):
+        """Every rank's per-case lists of rows -> the per-case lists over all voxels on master_rank ([] elsewhere): one
+        all-gather of the ``[cases, rows]`` accuracy matrix (on the device with NCCL, on the host with gloo)."""
+        if world == 1:
+            return [list(part) for part in local]
+        import torch
+        import torch.distributed as dist
+        dev = self._torch_device() if dist.get_backend() == "nccl" else torch.device("cpu")
+        parts = self.row_partition(self.num_voxels, world)
+        per = max(n for _, n in parts)
+        mine = torch.full((len(local), per), float("nan"), dtype=torch.float64)
+        for i, part in enumerate(local):
+            if part:
+                mine[i, :len(part)] = torch.tensor([a for _, a in part], dtype=torch.float64)
+        mine = mine.to(dev)
+        allv = [torch.empty_like(mine) for _ in range(world)]
+        dist.all_gather(allv, mine)
+        if rank != self.master_rank:
+            return [[] for _ in local]
+        host = torch.stack(allv).cpu().numpy()          # [world, cases, per]
+        return [[(int(s0 + k), host[r, i, k]) for r, (s0, n) in enumerate(parts) for k in range(n)]
+                for i in range(len(local))]
+
     def _gather(self, local, rank, world):
         if world == 1:
             return list(local)
@@ -287,26 +389,44 @@ class VoxelSelector:
         E = len(self.raw_data)
         return engine.sym_supported(E, self.epochs_per_subj) and self.num_voxels >= 512 * world
 
-    def _cv_block(self, K, s, nb, clf, on_gpu, folds):
-        """a7 tail + a8 for the unshrunk device kernels ``K`` of rows [s, s+nb)."""
-        t0 = time.time()
-        if on_gpu:
-            # shrink + cross validation without leaving the device (SURVEY §8f rank 1)
-            engine.shrink_kernels_(K)
-            acc = engine.svm_cv_precomputed(K, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
-                                            max_iter=clf.max_iter, folds=folds, shrinking=bool(clf.shrinking))
-            logger.debug('rows [%d, %d): GPU cv %.3f s', s, s + nb, time.time() - t0)
-            return [(int(s + k), acc[k]) for k in range(nb)]
-        kernels = K.cpu().numpy()
-        shrink_kernels_(kernels)
-        res = self._do_cross_validation(clf, kernels, (s, nb))
-        logger.debug('rows [%d, %d): host cv %.3f s', s, s + nb, time.time() - t0)
-        return res
+    def _precomputed_folds(self, clf, cases, E):
+        """Per case: the GPU fold problems of its cross validation of ``SVC(kernel='precomputed')``, or None for the host."""
+        return [engine.svm_folds_for(c.labels, c.num_folds, c.E)
+                if self.gpu_cv and engine.svm_cv_supported(clf, c.labels, c.num_folds, c.E,
+                                                           max_epochs=engine.SVM_WIDE_MAX_EPOCHS) else None
+                for c in cases]
 
-    def _score_rows_symmetric(self, start, n, clf):
+    def _cv_block(self, K, s, nb, clf, cases, folds):
+        """a7 tail + a8 for the unshrunk device kernels ``K`` of rows [s, s+nb), once per case (``folds``:
+        ``_precomputed_folds``).  Every epoch: shrunk in place; a held-out subject: compacted and shrunk out of place, so
+        ``K`` stays the block's unshrunk kernels for the next case."""
+        t0 = time.time()
+        out, host = [], None
+        for c, f in zip(cases, folds):
+            if f is not None:
+                # shrink + cross validation without leaving the device (SURVEY §8f rank 1)
+                if c.keep is None:
+                    engine.shrink_kernels_(K)
+                    Kc = K
+                else:
+                    Kc = engine.subset_kernels(K, c.keep, shrink=True)
+                acc = engine.svm_cv_precomputed(Kc, c.labels, c.num_folds, C=clf.C, tol=clf.tol,
+                                                max_iter=clf.max_iter, folds=f, shrinking=bool(clf.shrinking))
+                del Kc
+                out.append([(int(s + k), acc[k]) for k in range(nb)])
+                continue
+            if host is None:
+                host = K.cpu().numpy()
+            kernels = c.take(host, (1, 2))
+            shrink_kernels_(kernels)
+            out.append(self._do_cross_validation(clf, kernels, (s, nb), c.labels, c.num_folds))
+        logger.debug('rows [%d, %d): cv of %d cases %.3f s', s, s + nb, len(cases), time.time() - t0)
+        return out
+
+    def _score_rows_symmetric(self, start, n, clf, cases):
         """Single-mask path: this rank contracts its shard of the upper block triangle
         (engine.sym_row_partition), the [V, E, E] partial kernels are summed over the ranks, then every
-        rank cross-validates rows [start, start+n)."""
+        rank cross-validates rows [start, start+n), once per case."""
         import torch
         rank, world = self._world()
         op, _ = self._operands()
@@ -339,14 +459,13 @@ class VoxelSelector:
             K, k0 = mine, start
         else:
             k0 = 0
-        on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E,
-                                                         max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
-        folds = engine.svm_folds_for(self.labels, self.num_folds, E) if on_gpu else None
-        results = []
+        folds = self._precomputed_folds(clf, cases, E)
+        results = [[] for _ in cases]
         block = 8192
         for s in range(start, start + n, block):
             nb = min(block, start + n - s)
-            results += self._cv_block(K[s - k0:s - k0 + nb], s, nb, clf, on_gpu, folds)
+            for res, part in zip(results, self._cv_block(K[s - k0:s - k0 + nb], s, nb, clf, cases, folds)):
+                res += part
         return results
 
     def _plain_block(self, n, fp64_outputs=False, fp64_matrices=2):
@@ -367,89 +486,120 @@ class VoxelSelector:
             self._work = engine.Workspace(E, self.num_voxels2, block, rows_op.device)
         return block
 
-    def _feature_kind(self, clf, max_epochs=64):
+    def _all_epochs(self):
+        """``run()``'s one case: every epoch, the instance's labels and fold count."""
+        return [_Case(len(self.raw_data), self.labels, self.num_folds)]
+
+    def _feature_kind(self, clf, max_epochs=64, cases=None):
         """'linear' / 'rbf' when ``clf`` on the normalised correlation vectors is cross-validated on the GPU (fp64 kernel
-        matrices + the fp64 solver) at up to ``max_epochs`` epochs, else None.  mask_self is not applied to the features
-        by the host path, so that combination stays there."""
+        matrices + the fp64 solver) at up to ``max_epochs`` epochs for every case (default: ``run()``'s), else None.
+        mask_self is not applied to the features by the host path, so that combination stays there."""
         if not self.gpu_cv or self.mask_self:
             return None
-        return engine.svc_feature_kind(clf, self.labels, self.num_folds, len(self.raw_data), max_epochs=max_epochs)
+        kinds = {engine.svc_feature_kind(clf, c.labels, c.num_folds, c.E, max_epochs=max_epochs)
+                 for c in (cases or self._all_epochs())}
+        return kinds.pop() if len(kinds) == 1 else None
 
-    def _scale_ok(self, clf):
+    def _scale_ok(self, clf, cases=None):
         """True when ``SVC(kernel='rbf', gamma='scale')`` on the normalised correlation vectors is cross-validated on the
-        GPU with per-fold gammas (engine.svm_cv_scale), under the conditions of ``_feature_kind``."""
+        GPU with per-fold gammas (engine.svm_cv_scale) for every case, under the conditions of ``_feature_kind``."""
         if not self.gpu_cv or self.mask_self:
             return False
-        return engine.svc_scale_supported(clf, self.labels, self.num_folds, len(self.raw_data))
+        return all(engine.svc_scale_supported(clf, c.labels, c.num_folds, c.E) for c in (cases or self._all_epochs()))
 
-    def _score_rows_scale(self, start, n, clf):
+    def _score_rows_scale(self, start, n, clf, cases):
         """SVC(kernel='rbf', gamma='scale') on the features of rows [start, start+n): G, D and the per-sample moments of
-        every row (engine.feature_gram_wide), then per fold the gamma of its training samples, its rbf kernels and the fp64
-        solver (engine.svm_cv_scale).  The voxels whose gamma may differ from scikit-learn's are scored on the host."""
+        every row (engine.feature_gram_wide), then per case (compacted to its epochs) and fold the gamma of its training
+        samples, its rbf kernels and the fp64 solver (engine.svm_cv_scale).  The voxels whose gamma may differ from
+        scikit-learn's are scored on the host."""
+        import torch
         rows_op, cols_op = self._operands()
-        E = rows_op.E
-        folds = engine.svm_folds_for(self.labels, self.num_folds, E)
-        block = self._plain_block(n, fp64_outputs=True, fp64_matrices=4)
-        results = []
+        folds = [engine.svm_folds_for(c.labels, c.num_folds, c.E) for c in cases]
+        held_out = any(c.keep is not None for c in cases)
+        # a held-out case also holds its compacted G and D
+        block = self._plain_block(n, fp64_outputs=True, fp64_matrices=6 if held_out else 4)
+        results = [[] for _ in cases]
         for s in range(start, start + n, block):
             nb = min(block, start + n - s)
             G, D, moments = engine.feature_gram_wide(rows_op, cols_op, s, nb, self.epochs_per_subj, work=self._work)
-            acc, flagged = engine.svm_cv_scale(G, D, moments, self.num_voxels2, self.labels, self.num_folds, C=clf.C,
-                                               tol=clf.tol, max_iter=clf.max_iter, shrinking=bool(clf.shrinking),
-                                               folds=folds)
+            for c, f, res in zip(cases, folds, results):
+                if c.keep is None:
+                    Gc, Dc, mc = G, D, moments
+                else:
+                    Gc, Dc = engine.subset_kernels(G, c.keep), engine.subset_kernels(D, c.keep)
+                    mc = moments.index_select(1, torch.as_tensor(c.keep, device=moments.device))
+                acc, flagged = engine.svm_cv_scale(Gc, Dc, mc, self.num_voxels2, c.labels, c.num_folds, C=clf.C,
+                                                   tol=clf.tol, max_iter=clf.max_iter, shrinking=bool(clf.shrinking),
+                                                   folds=f)
+                del Gc, Dc, mc
+                part = [(int(s + k), acc[k]) for k in range(nb)]
+                for k in np.flatnonzero(flagged):
+                    task = (int(s + k), 1)
+                    part[k] = (self._voxel_scoring(task, clf) if c.keep is None
+                               else self._host_scoring(task, clf, [c])[0])[0]
+                if flagged.any():
+                    logger.info('rows [%d, %d): %d voxels scored on the host (gamma=\'scale\' variance check)', s,
+                                s + nb, int(flagged.sum()))
+                res += part
             del G, D, moments
-            part = [(int(s + k), acc[k]) for k in range(nb)]
-            for k in np.flatnonzero(flagged):
-                part[k] = self._voxel_scoring((int(s + k), 1), clf)[0]
-            if flagged.any():
-                logger.info('rows [%d, %d): %d voxels scored on the host (gamma=\'scale\' variance check)', s, s + nb,
-                            int(flagged.sum()))
-            results += part
         return results
 
     def _score_rows(self, start, n, clf):
         """GPU stages for rows [start, start+n) in HBM-sized blocks, then the cross validation (GPU or host)."""
-        import torch
+        return self._score_cases(start, n, clf, self._all_epochs())[0]
+
+    def _score_cases(self, start, n, clf, cases):
+        """``_score_rows`` for every case of ``cases`` from one kernel build: one list of ``(voxel_id, accuracy)`` per
+        case.  The build and its route are ``run()``'s over all E epochs; each case then cross-validates its epochs."""
         rows_op, cols_op = self._operands()
         E = rows_op.E
-        results = []
+        results = [[] for _ in cases]
+        held_out = any(c.keep is not None for c in cases)
         if _is_precomputed_svc(clf) and self._symmetric_ok():
-            return self._score_rows_symmetric(start, n, clf)
-        kind = None if _is_precomputed_svc(clf) else self._feature_kind(clf, max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
+            return self._score_rows_symmetric(start, n, clf, cases)
+        kind = None if _is_precomputed_svc(clf) else self._feature_kind(clf, engine.SVM_WIDE_MAX_EPOCHS, cases)
         if kind is not None:
             # SVC(kernel='linear' | 'rbf') on the features: the fp64 kernels of the features give libsvm's iterations and
             # decisions (DESIGN.md §3.8); gamma='auto' is scikit-learn's 1 / n_features
             gamma = None if kind == 'linear' else (1.0 / self.num_voxels2 if clf.gamma == 'auto' else float(clf.gamma))
             wide = E > 64
-            folds = engine.svm_folds_for(self.labels, self.num_folds, E)
+            folds = [engine.svm_folds_for(c.labels, c.num_folds, c.E) for c in cases]
             feature_kernels = engine.feature_kernels_f64_wide if wide else engine.feature_kernels_f64
-            block = self._plain_block(n, fp64_outputs=wide)
+            # a held-out case also holds its compacted K_fit and K_pred
+            block = self._plain_block(n, fp64_outputs=wide, fp64_matrices=4 if held_out else 2)
             for s in range(start, start + n, block):
                 nb = min(block, start + n - s)
                 K_fit, K_pred = feature_kernels(rows_op, cols_op, s, nb, self.epochs_per_subj, kind, gamma,
                                                 work=self._work)
-                acc = engine.svm_cv_f64(K_fit, K_pred, self.labels, self.num_folds, C=clf.C, tol=clf.tol,
-                                        max_iter=clf.max_iter, shrinking=bool(clf.shrinking), folds=folds)
+                for c, f, res in zip(cases, folds, results):
+                    if c.keep is None:
+                        Kf, Kp = K_fit, K_pred
+                    else:
+                        Kf = engine.subset_kernels(K_fit, c.keep)
+                        Kp = Kf if K_pred is K_fit else engine.subset_kernels(K_pred, c.keep)
+                    acc = engine.svm_cv_f64(Kf, Kp, c.labels, c.num_folds, C=clf.C, tol=clf.tol,
+                                            max_iter=clf.max_iter, shrinking=bool(clf.shrinking), folds=f)
+                    del Kf, Kp
+                    res += [(int(s + k), acc[k]) for k in range(nb)]
                 del K_fit, K_pred
-                results += [(int(s + k), acc[k]) for k in range(nb)]
         elif _is_precomputed_svc(clf):
             fused = engine.fused_supported(E, self.epochs_per_subj)
             block = self._plain_block(n)
-            on_gpu = self.gpu_cv and engine.svm_cv_supported(clf, self.labels, self.num_folds, E,
-                                                             max_epochs=engine.SVM_WIDE_MAX_EPOCHS)
-            folds = engine.svm_folds_for(self.labels, self.num_folds, E) if on_gpu else None
+            folds = self._precomputed_folds(clf, cases, E)
             for s in range(start, start + n, block):
                 nb = min(block, start + n - s)
                 K = engine.voxel_kernels(rows_op, cols_op, s, nb, self.epochs_per_subj,
                                          flags=self._flags(fused), work=self._work)
-                results += self._cv_block(K, s, nb, clf, on_gpu, folds)
-        elif self._scale_ok(clf):
-            results = self._score_rows_scale(start, n, clf)
+                for res, part in zip(results, self._cv_block(K, s, nb, clf, cases, folds)):
+                    res += part
+        elif self._scale_ok(clf, cases):
+            results = self._score_rows_scale(start, n, clf, cases)
         else:
             unit = max(1, min(self.voxel_unit, n))
             for s in range(start, start + n, unit):
                 nb = min(unit, start + n - s)
-                results += self._voxel_scoring((s, nb), clf)
+                for res, part in zip(results, self._host_scoring((s, nb), clf, cases)):
+                    res += part
         return results
 
     # ------------------------------------------------------------------ reference stage methods
@@ -487,40 +637,53 @@ class VoxelSelector:
             return shrink_kernels_(kernels)
         return corr
 
-    def _do_cross_validation(self, clf, data, task):
-        """a8 (voxelselector.py:423-465): voxelwise cross validation on the host."""
+    def _do_cross_validation(self, clf, data, task, labels=None, num_folds=None):
+        """a8 (voxelselector.py:423-465): voxelwise cross validation on the host, with ``labels`` and ``num_folds``
+        (default: the instance's)."""
         time1 = time.time()
+        labels = self.labels if labels is None else labels
+        num_folds = self.num_folds if num_folds is None else num_folds
         n = task[1]
         if _is_precomputed_svc(clf) and self.use_multiprocessing and n > 1:
             nproc = int(self.process_num)
             chunk = max(1, int(math.ceil(n / float(nproc * 4))))
-            inlist = [(clf, np.arange(c, min(n, c + chunk)) + task[0], self.num_folds,
-                       data[c:min(n, c + chunk)], self.labels) for c in range(0, n, chunk)]
+            inlist = [(clf, np.arange(c, min(n, c + chunk)) + task[0], num_folds,
+                       data[c:min(n, c + chunk)], labels) for c in range(0, n, chunk)]
             with multiprocessing.Pool(nproc) as pool:
                 parts = pool.starmap(_cv_chunk, inlist)
             results = [r for part in parts for r in part]
         else:
-            results = [_cross_validation_for_one_voxel(clf, i + task[0], self.num_folds,
-                                                       data[i, :, :], self.labels)
+            results = [_cross_validation_for_one_voxel(clf, i + task[0], num_folds,
+                                                       data[i, :, :], labels)
                        for i in range(n)]
         logger.debug('cross validation for %d voxels, takes %.2f s', n, time.time() - time1)
         return results
 
     def _voxel_scoring(self, task, clf):
         """One task ``(start, n)`` through the 3-stage pipeline of voxelselector.py:467-516."""
-        import torch
+        return self._host_scoring(task, clf, self._all_epochs())[0]
+
+    def _host_scoring(self, task, clf, cases):
+        """``_voxel_scoring`` once per case: the task's kernels (shrunk per case on its epochs) or normalised
+        correlations are computed once over all epochs, then each case cross-validates its epochs on the host."""
         time1 = time.time()
         rows_op, cols_op = self._operands()
-        if _is_precomputed_svc(clf):
+        precomputed = _is_precomputed_svc(clf)
+        if precomputed:
             fused = engine.fused_supported(rows_op.E, self.epochs_per_subj)
             K = engine.voxel_kernels(rows_op, cols_op, task[0], task[1], self.epochs_per_subj,
                                      flags=self._flags(fused))
-            data = shrink_kernels_(K.cpu().numpy())
+            data = K.cpu().numpy()
         else:
             corr = engine.corr_block(rows_op, cols_op, task[0], task[1], layout=0)
             corr = corr.contiguous()
             engine.within_subject_norm_(corr, self.epochs_per_subj)
             data = corr.cpu().numpy()
-        results = self._do_cross_validation(clf, data, task)
+        results = []
+        for c in cases:
+            d = c.take(data, (1, 2) if precomputed else (1,))
+            if precomputed:
+                shrink_kernels_(d)
+            results.append(self._do_cross_validation(clf, d, task, c.labels, c.num_folds))
         logger.info('task %d takes %.2f s', int(task[0] / self.voxel_unit), time.time() - time1)
         return results

@@ -200,6 +200,17 @@ int fcma_classifier_kernel_sym(const void *op, int precision, int E, int T, long
  * int[nv]) receives len(str(int(K[0][0]))) */
 int fcma_shrink_kernels(float *K_dev, long nv, int E, int *digits_dev, void *stream);
 
+/* the kernels of a subset of the epochs, out of place: out_dev[v][a][b] = K_dev[v][keep[a]][keep[b]], a contiguous
+ * [nv][E_keep][E_keep] array (leave-one-subject-out: the full run's kernels without one subject's rows and columns).
+ * keep_host: E_keep strictly increasing epoch indices in [0, E), E <= 256, read on the host and passed to the kernel by
+ * value.  shrink != 0 also applies fcma_shrink_kernels' decimal shrink, its digits counted on the compacted
+ * out[v][0][0]; digits_dev (optional, int[nv]) receives them.  The output must not overlap K_dev. */
+int fcma_subset_kernels(const float *K_dev, long nv, int E, const int *keep_host, int E_keep, float *out_dev,
+                        int shrink, int *digits_dev, void *stream);
+/* the same gather on fp64 kernels (K_fit, K_pred, G and D of the feature route), without a shrink */
+int fcma_subset_kernels_f64(const double *K_dev, long nv, int E, const int *keep_host, int E_keep, double *out_dev,
+                            void *stream);
+
 /* batched cross-validation of SVC(kernel='precomputed') (binary C-SVC, libsvm SMO restated from
  * scikit-learn's sklearn/svm/src/libsvm/svm.cpp) on nv kernels [E][E]: folds_host points to nfolds
  * structs {int n_train, n_pos, n_test, pad; int train_idx[64]; int test_idx[64]; unsigned char test_pos[64]}
