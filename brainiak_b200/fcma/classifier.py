@@ -36,6 +36,17 @@ def _is_precomputed_svc(clf):
     return isinstance(clf, sklearn.svm.SVC) and clf.kernel == 'precomputed'
 
 
+# the kernel matrix of more than 64 samples is formed by k_syrk_simt, which holds 64 (E + 1) floats of shared memory
+# per block, at most 200 KB
+MAX_KERNEL_SAMPLES = 799
+
+
+def _check_kernel_samples(E, what):
+    if E > MAX_KERNEL_SAMPLES:
+        raise ValueError("%s: %d samples, but the kernel matrix of SVC(kernel='precomputed') is limited to %d samples"
+                         % (what, E, MAX_KERNEL_SAMPLES))
+
+
 class Classifier(BaseEstimator):
     """Correlation-based classification component of FCMA (H100 engine).
 
@@ -47,6 +58,10 @@ class Classifier(BaseEstimator):
         operand precision of the correlation contraction ('fp32' = fp32-faithful 3-product split,
         see VoxelSelector).
     device: optional CUDA device
+
+    With ``SVC(kernel='precomputed')`` the kernel matrix holds at most ``MAX_KERNEL_SAMPLES`` = 799 samples: the
+    samples of ``fit``, and after a fit in portions (``num_processed_voxels`` below the larger mask) the training samples
+    of fit's subjects plus the samples given to ``predict`` / ``decision_function``.  More raise ``ValueError``.
 
     Attributes (classifier.py:68-114)
     ----------
@@ -154,8 +169,9 @@ class Classifier(BaseEstimator):
         the second item is the ``[1, E, rows*V2]`` features of the LAST portion, kept only when a
         single portion covers all voxels (it becomes ``training_data_``)."""
         import torch
-        op1, op2 = self._pack_pair(X1, X2)
         E = self.num_samples_
+        _check_kernel_samples(E, "fit")
+        op1, op2 = self._pack_pair(X1, X2)
         num_voxels2 = X2[0].shape[1]
         single = self.num_processed_voxels >= self.num_voxels_
         normalized_corr_data = None
@@ -207,9 +223,14 @@ class Classifier(BaseEstimator):
             else:
                 self.training_data_ = None
                 # references (no copies) to the raw training epochs: what streamed prediction needs instead of the
-                # [n_train, V1*V2] features
+                # [n_train, V1*V2] features.  fit normalised the training samples within subjects of epochs_per_subj
+                # over all fit samples, so a subject cut by n_train is kept whole: its first samples' features depend
+                # on the fit-time test samples that share the subject
                 n_train = num_training_samples if num_training_samples is not None else self.num_samples_
-                self._train_raw_ = (list(X1[:n_train]), list(X2[:n_train]))
+                eps = self.epochs_per_subj
+                n_span = n_train if eps <= 1 else min(self.num_samples_, -(-n_train // eps) * eps)
+                self._train_raw_ = (list(X1[:n_span]), list(X2[:n_span]))
+                self._num_train_ = n_train
             logger.debug('kernel computation done')
         return data
 
@@ -279,14 +300,18 @@ class Classifier(BaseEstimator):
         the correlation block ``[samples, rows, V2]`` (a9), the training part is normalised within subject with
         ``epochs_per_subj`` as ``fit`` does (classifier.py:325-327), the test part over all test samples as ``predict``
         does (classifier.py:554-556), and ``K += Z Z^T`` accumulates the Gram matrix over the portions (a11); its
-        test x train block, scaled with the ``num_digits_`` of the training kernel, is the similarity."""
+        test x train block, scaled with the ``num_digits_`` of the training kernel, is the similarity.  The training
+        part is the fit samples up to the end of the subject of the last training sample (``_train_raw_``), so every
+        training sample is z-scored with the same epochs as in ``fit``; only the first ``n_train`` columns are used."""
         import torch
         tr1, tr2 = self._train_raw_
-        n_train, n_test = len(tr1), len(X1)
+        n_span, n_test = len(tr1), len(X1)
+        n_train = getattr(self, "_num_train_", n_span)
         if tr1[0].shape[1] != X1[0].shape[1]:        # fit() may have swapped the masks so that X1 is the larger one
             tr1, tr2 = tr2, tr1
+        Es = n_span + n_test
+        _check_kernel_samples(Es, "the training samples of fit's subjects and the test samples")
         op1, op2 = self._pack_pair(list(tr1) + list(X1), list(tr2) + list(X2))
-        Es = n_train + n_test
         V1, V2 = op1.V, op2.V
         rows = int(max(1, min(self.num_processed_voxels, V1, max_bytes // (Es * V2 * 4))))
         K = torch.zeros((Es, Es), dtype=torch.float32, device=op1.device)
@@ -294,11 +319,11 @@ class Classifier(BaseEstimator):
             nb = min(rows, V1 - start)
             corr = engine.corr_block(op1, op2, start, nb, layout=1)                    # [Es, nb, V2]
             if self.epochs_per_subj > 1:
-                engine.within_subject_norm_(corr[:n_train].view(1, n_train, nb * V2), self.epochs_per_subj)
+                engine.within_subject_norm_(corr[:n_span].view(1, n_span, nb * V2), self.epochs_per_subj)
             if n_test > 1:
-                engine.within_subject_norm_(corr[n_train:].view(1, n_test, nb * V2), n_test)
+                engine.within_subject_norm_(corr[n_span:].view(1, n_test, nb * V2), n_test)
             engine.kernel_matrices(corr.view(1, Es, nb * V2), beta=1.0, out=K, sum_over_rows=True)
-        data = K[n_train:, :n_train].cpu().numpy()
+        data = K[n_span:, :n_train].cpu().numpy()
         if self.num_digits_ > 2:
             data *= 10 ** (2 - self.num_digits_)
         logger.debug('streamed similarity vectors computation done')
